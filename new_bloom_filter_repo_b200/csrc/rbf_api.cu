@@ -724,6 +724,17 @@ static int stream_fill_pairs(rbf_stream* s, uint32_t first, uint32_t count, cons
     return RBF_OK;
 }
 
+// Pairs of a consecutive run of frames (pairs[t].curr == pairs[t+1].prev) let K1 read each frame once instead of twice; its bulk
+// copies also need 16 B aligned frames, which cudaMalloc and the 256-byte frame stride give.
+static bool pairs_form_chain(const PairJob* h, uint32_t count) {
+    if (count < 2) return false;
+    for (uint32_t i = 0; i < count; i++) {
+        if (((uintptr_t)h[i].prev | (uintptr_t)h[i].curr) & 15u) return false;
+        if (i + 1 < count && h[i].curr != h[i + 1].prev) return false;
+    }
+    return true;
+}
+
 struct RangeTotals {
     uint32_t total_cent = 0, coded_pairs = 0, max_l = 0;
 };
@@ -798,7 +809,8 @@ static int stream_encode_range(rbf_stream* s, uint32_t first, uint32_t count, ui
     CK(c, cudaMemsetAsync(s->d_resid + first, 0, 4 * (size_t)count, c->st));
     if (record_events) { s->staged = false; CK(c, cudaEventRecord(s->ev[0], c->st)); }
     LAUNCH(c, launch_threshold(s->d_pairs + first, (int)count, n, (int)s->C, (int)s->S, thr_int, s->mask_mode, s->gray_mode,
-                               s->d_ones + first, s->d_resid + first, c->k1_variant, c->sm_count, c->k1_ctas_per_sm, c->st));
+                               s->d_ones + first, s->d_resid + first, c->k1_variant, pairs_form_chain(s->h_pairs + first, count),
+                               c->sm_count, c->k1_ctas_per_sm, c->st));
     if (c->k1_variant == 1 && !s->gray_mode) c->launches++;              // tail kernel
     if (record_events) CK(c, cudaEventRecord(s->ev[1], c->st));
     CK(c, cudaMemcpyAsync(s->h_ones + first, s->d_ones + first, 4 * (size_t)count, cudaMemcpyDeviceToHost, c->st));
@@ -868,7 +880,7 @@ static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t
     for (uint32_t r = 0; r < R; r++) {
         const uint32_t f = lo[r], cnt = lo[r + 1] - lo[r];
         LAUNCH(c, launch_threshold(s->d_pairs + f, (int)cnt, n, (int)s->C, (int)s->S, thr_int, s->mask_mode, s->gray_mode, s->d_ones + f,
-                                   s->d_resid + f, c->k1_variant, c->sm_count, k1_cap, c->st_k1));
+                                   s->d_resid + f, c->k1_variant, pairs_form_chain(s->h_pairs + f, cnt), c->sm_count, k1_cap, c->st_k1));
         if (c->k1_variant == 1 && !s->gray_mode) c->launches++;
         CK(c, cudaMemcpyAsync(s->h_ones + f, s->d_ones + f, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, c->st_k1));
         CK(c, cudaMemcpyAsync(s->h_resid + f, s->d_resid + f, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, c->st_k1));

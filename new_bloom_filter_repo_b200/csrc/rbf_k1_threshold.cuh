@@ -2,9 +2,13 @@
 #pragma once
 
 // ------------------------------------------------------------------------------------------
-// K1: threshold + popcount.  One thread = 32 consecutive pixels = one mask word; the pixel
-// bytes of a warp are staged in shared memory (see stage_warp), 2*PB 16 B copies per lane and frame.
+// K1: threshold + popcount.  One thread = 32 consecutive pixels = one mask word (threshold_word).
 // PB = bytes per pixel (channels * sample bytes), S = sample bytes; Y is the first sample.
+//   k_threshold_sweep  pairs that form a chain (consecutive frames, the benchmark's case): each frame is read from HBM once
+//                      (2.87 ms per 299 4K pairs on an H100 80GB HBM3 at 400 W, 0.81 of the 3.35 TB/s data-sheet bandwidth)
+//   k_threshold        any pair list: the pixel bytes of a warp are staged in shared memory (see stage_warp), 2*PB 16 B
+//                      copies per lane and frame; a frame shared by two pairs is read twice (4.33 ms on the same card)
+//   k_threshold_tma    k1_variant=1
 // ------------------------------------------------------------------------------------------
 template <int PB, int S>
 __device__ __forceinline__ int absdiff_sample(uint32_t a, uint32_t b) {
@@ -74,6 +78,107 @@ __device__ __forceinline__ void stage_warp(uint8_t* dst, const uint8_t* src, uin
                      : "memory");
 }
 
+// The threshold in the forms the per-word compare uses
+struct K1Thr {
+    int thr, any_mode;
+    uint32_t thr4, gt_or, gt_and, any_mask;
+};
+__device__ __forceinline__ K1Thr k1_thr(int thr, int any_mode) {
+    K1Thr t;
+    t.thr = thr;
+    t.any_mode = any_mode;
+    t.thr4 = (uint32_t)(thr < 0 ? 0 : (thr > 254 ? 254 : thr)) * 0x01010101u;
+    t.gt_or = thr < 0 ? 0xffffffffu : 0u;
+    t.gt_and = thr > 254 ? 0u : 0xffffffffu;
+    t.any_mask = any_mode ? 0xfu : 0u;
+    return t;
+}
+
+// One mask word: the 32 whole pixels at pa (prev) and pb (curr), in shared memory (staged) or global memory, both 16 B aligned.
+// m = mask bits, r = residual bits (some byte of the pixel differs, mask bit clear).
+template <int PB, int S, bool GRAY>
+__device__ __forceinline__ void threshold_word(const uint8_t* pa, const uint8_t* pb, bool staged, const K1Thr& t, uint32_t& m,
+                                               uint32_t& r) {
+    m = 0; r = 0;
+    if (PB == 3 && S == 1 && !GRAY) {
+        uint32_t A[24], B[24];
+#pragma unroll
+        for (int j = 0; j < 3; j++) load32B(pa + 32 * j, A + 8 * j, staged);
+#pragma unroll
+        for (int j = 0; j < 3; j++) load32B(pb + 32 * j, B + 8 * j, staged);
+#pragma unroll
+        for (int g = 0; g < 8; g++) {
+            uint32_t nm, nd;
+            yuv8_group4(A[3 * g], A[3 * g + 1], A[3 * g + 2], B[3 * g], B[3 * g + 1], B[3 * g + 2], t.thr4, t.gt_or, t.gt_and, nm, nd);
+            nm |= nd & t.any_mask;
+            m |= nm << (4 * g);
+            r |= (nd & ~nm) << (4 * g);
+        }
+    } else {
+        constexpr int NV = PB;                     // 32 B loads per 32 pixels
+        constexpr int HV = (NV > 3) ? NV / 2 : NV; // at most 3 in flight per frame
+        constexpr int HALVES = NV / HV;
+        constexpr int PXH = 32 / HALVES;
+#pragma unroll
+        for (int hf = 0; hf < HALVES; hf++) {
+            uint32_t A[8 * HV], B[8 * HV];
+            const uint32_t ho = (uint32_t)(hf * PXH) * PB;
+#pragma unroll
+            for (int j = 0; j < HV; j++) load32B(pa + ho + 32 * j, A + 8 * j, staged);
+#pragma unroll
+            for (int j = 0; j < HV; j++) load32B(pb + ho + 32 * j, B + 8 * j, staged);
+#pragma unroll
+            for (int k = 0; k < PXH; k++) {
+                const int o = k * PB;              // byte offset of the pixel (compile-time)
+                const uint32_t smask = (S == 1) ? 0xffu : 0xffffu;
+                uint32_t ya = (A[o >> 2] >> (8 * (o & 3))) & smask;
+                uint32_t yb = (B[o >> 2] >> (8 * (o & 3))) & smask;
+                if (GRAY) {                        // samples 1 and 2 of the pixel (compile-time offsets; S == 2 samples are 2-aligned)
+                    const int p1 = o + S, p2 = o + 2 * S;
+                    const uint32_t a1 = (A[p1 >> 2] >> (8 * (p1 & 3))) & smask, a2 = (A[p2 >> 2] >> (8 * (p2 & 3))) & smask;
+                    const uint32_t b1 = (B[p1 >> 2] >> (8 * (p1 & 3))) & smask, b2 = (B[p2 >> 2] >> (8 * (p2 & 3))) & smask;
+                    ya = bgr2gray_fixed(ya, a1, a2);
+                    yb = bgr2gray_fixed(yb, b1, b2);
+                }
+                uint32_t anyd = 0;                 // any byte of the pixel differs
+#pragma unroll
+                for (int q = 0; q < PB; q++) {
+                    const int oq = o + q;
+                    anyd |= ((A[oq >> 2] ^ B[oq >> 2]) >> (8 * (oq & 3))) & 0xffu;
+                }
+                const uint32_t bit = ((absdiff_sample<PB, S>(ya, yb) > t.thr) || (t.any_mode && anyd != 0u)) ? 1u : 0u;
+                m |= bit << (hf * PXH + k);
+                r |= ((anyd != 0u && bit == 0u) ? 1u : 0u) << (hf * PXH + k);
+            }
+        }
+    }
+}
+
+// The ragged last word of a frame: the first nvalid (< 32) pixels at a (prev) and b (curr) in global memory, scalar loads.
+template <int PB, int S, bool GRAY>
+__device__ __forceinline__ void threshold_word_tail(const uint8_t* pa, const uint8_t* pb, uint32_t nvalid, const K1Thr& t, uint32_t& m,
+                                                    uint32_t& r) {
+    m = 0; r = 0;
+    for (uint32_t k = 0; k < nvalid; k++) {
+        const uint8_t* a = pa + (size_t)k * PB;
+        const uint8_t* b = pb + (size_t)k * PB;
+        uint32_t ya = a[0], yb = b[0];
+        if (S == 2) { ya |= (uint32_t)a[1] << 8; yb |= (uint32_t)b[1] << 8; }
+        if (GRAY) {
+            uint32_t a1 = a[S], a2 = a[2 * S], b1 = b[S], b2 = b[2 * S];
+            if (S == 2) { a1 |= (uint32_t)a[3] << 8; a2 |= (uint32_t)a[5] << 8; b1 |= (uint32_t)b[3] << 8; b2 |= (uint32_t)b[5] << 8; }
+            ya = bgr2gray_fixed(ya, a1, a2);
+            yb = bgr2gray_fixed(yb, b1, b2);
+        }
+        uint32_t anyd = 0;
+        for (int q = 0; q < PB; q++) anyd |= (uint32_t)(a[q] ^ b[q]);
+        const uint32_t bit = ((absdiff_sample<PB, S>(ya, yb) > t.thr) || (t.any_mode && anyd != 0u)) ? 1u : 0u;
+        m |= bit << k;
+        r |= ((anyd != 0u && bit == 0u) ? 1u : 0u) << k;
+    }
+}
+
+// K1 for any list of pairs: grid (bx, pairs), each CTA grid-strides over the mask words of its pair.
 template <int PB, int S, bool GRAY = false>
 __global__ void __launch_bounds__(K1_THREADS) k_threshold(const PairJob* __restrict__ pairs, uint32_t npix, int thr, int any_mode,
                                                           uint32_t* __restrict__ ones, uint32_t* __restrict__ resid) {
@@ -82,15 +187,13 @@ __global__ void __launch_bounds__(K1_THREADS) k_threshold(const PairJob* __restr
     const PairJob pj = pairs[blockIdx.y];
     const uint32_t nwords = (npix + 31u) >> 5;
     uint32_t cnt_ones = 0, cnt_res = 0;
-    const uint32_t thr4 = (uint32_t)(thr < 0 ? 0 : (thr > 254 ? 254 : thr)) * 0x01010101u;
-    const uint32_t gt_or = thr < 0 ? 0xffffffffu : 0u, gt_and = thr > 254 ? 0u : 0xffffffffu;
-    const uint32_t any_mask = any_mode ? 0xfu : 0u;
+    const K1Thr t = k1_thr(thr, any_mode);
     const uint32_t lane = threadIdx.x & 31u;
     uint8_t* const sa = k1_stage + (threadIdx.x >> 5) * 2048 * PB;
     uint8_t* const sb = sa + 1024 * PB;
     for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < nwords; w += gridDim.x * blockDim.x) {
         const uint32_t px0 = w << 5;
-        uint32_t m = 0, r = 0;
+        uint32_t m, r;
         const bool staged = (uint64_t)((w | 31u) + 1u) * 32u <= npix;          // warp-uniform: the block stride is a multiple of 32
         if (staged) {
             __syncwarp();                                                    // the lanes have read the previous iteration's slice
@@ -100,82 +203,11 @@ __global__ void __launch_bounds__(K1_THREADS) k_threshold(const PairJob* __restr
             asm volatile("cp.async.wait_all;" ::: "memory");
             __syncwarp();
         }
-        if (px0 + 32u <= npix) {
-            if (PB == 3 && S == 1 && !GRAY) {
-                uint32_t A[24], B[24];
-                const uint8_t* pa = staged ? sa + lane * 96u : pj.prev + (size_t)px0 * 3;
-                const uint8_t* pb = staged ? sb + lane * 96u : pj.curr + (size_t)px0 * 3;
-#pragma unroll
-                for (int j = 0; j < 3; j++) load32B(pa + 32 * j, A + 8 * j, staged);
-#pragma unroll
-                for (int j = 0; j < 3; j++) load32B(pb + 32 * j, B + 8 * j, staged);
-#pragma unroll
-                for (int g = 0; g < 8; g++) {
-                    uint32_t nm, nd;
-                    yuv8_group4(A[3 * g], A[3 * g + 1], A[3 * g + 2], B[3 * g], B[3 * g + 1], B[3 * g + 2], thr4, gt_or, gt_and, nm, nd);
-                    nm |= nd & any_mask;
-                    m |= nm << (4 * g);
-                    r |= (nd & ~nm) << (4 * g);
-                }
-            } else {
-                constexpr int NV = PB;                     // 32 B loads per 32 pixels
-                constexpr int HV = (NV > 3) ? NV / 2 : NV; // at most 3 in flight per frame
-                constexpr int HALVES = NV / HV;
-                constexpr int PXH = 32 / HALVES;
-#pragma unroll
-                for (int hf = 0; hf < HALVES; hf++) {
-                    uint32_t A[8 * HV], B[8 * HV];
-                    const uint32_t ho = (uint32_t)(hf * PXH) * PB;
-                    const uint8_t* pa = staged ? sa + lane * 32u * PB + ho : pj.prev + (size_t)px0 * PB + ho;
-                    const uint8_t* pb = staged ? sb + lane * 32u * PB + ho : pj.curr + (size_t)px0 * PB + ho;
-#pragma unroll
-                    for (int j = 0; j < HV; j++) load32B(pa + 32 * j, A + 8 * j, staged);
-#pragma unroll
-                    for (int j = 0; j < HV; j++) load32B(pb + 32 * j, B + 8 * j, staged);
-#pragma unroll
-                    for (int k = 0; k < PXH; k++) {
-                        const int o = k * PB;              // byte offset of the pixel (compile-time)
-                        const uint32_t smask = (S == 1) ? 0xffu : 0xffffu;
-                        uint32_t ya = (A[o >> 2] >> (8 * (o & 3))) & smask;
-                        uint32_t yb = (B[o >> 2] >> (8 * (o & 3))) & smask;
-                        if (GRAY) {                        // samples 1 and 2 of the pixel (compile-time offsets; S == 2 samples are 2-aligned)
-                            const int p1 = o + S, p2 = o + 2 * S;
-                            const uint32_t a1 = (A[p1 >> 2] >> (8 * (p1 & 3))) & smask, a2 = (A[p2 >> 2] >> (8 * (p2 & 3))) & smask;
-                            const uint32_t b1 = (B[p1 >> 2] >> (8 * (p1 & 3))) & smask, b2 = (B[p2 >> 2] >> (8 * (p2 & 3))) & smask;
-                            ya = bgr2gray_fixed(ya, a1, a2);
-                            yb = bgr2gray_fixed(yb, b1, b2);
-                        }
-                        uint32_t anyd = 0;                 // any byte of the pixel differs
-#pragma unroll
-                        for (int q = 0; q < PB; q++) {
-                            const int oq = o + q;
-                            anyd |= ((A[oq >> 2] ^ B[oq >> 2]) >> (8 * (oq & 3))) & 0xffu;
-                        }
-                        const uint32_t bit = ((absdiff_sample<PB, S>(ya, yb) > thr) || (any_mode && anyd != 0u)) ? 1u : 0u;
-                        m |= bit << (hf * PXH + k);
-                        r |= ((anyd != 0u && bit == 0u) ? 1u : 0u) << (hf * PXH + k);
-                    }
-                }
-            }
-        } else {                                        // ragged last word: scalar loads
-            for (uint32_t k = 0; k < 32u && px0 + k < npix; k++) {
-                const uint8_t* a = pj.prev + (size_t)(px0 + k) * PB;
-                const uint8_t* b = pj.curr + (size_t)(px0 + k) * PB;
-                uint32_t ya = a[0], yb = b[0];
-                if (S == 2) { ya |= (uint32_t)a[1] << 8; yb |= (uint32_t)b[1] << 8; }
-                if (GRAY) {
-                    uint32_t a1 = a[S], a2 = a[2 * S], b1 = b[S], b2 = b[2 * S];
-                    if (S == 2) { a1 |= (uint32_t)a[3] << 8; a2 |= (uint32_t)a[5] << 8; b1 |= (uint32_t)b[3] << 8; b2 |= (uint32_t)b[5] << 8; }
-                    ya = bgr2gray_fixed(ya, a1, a2);
-                    yb = bgr2gray_fixed(yb, b1, b2);
-                }
-                uint32_t anyd = 0;
-                for (int q = 0; q < PB; q++) anyd |= (uint32_t)(a[q] ^ b[q]);
-                const uint32_t bit = ((absdiff_sample<PB, S>(ya, yb) > thr) || (any_mode && anyd != 0u)) ? 1u : 0u;
-                m |= bit << k;
-                r |= ((anyd != 0u && bit == 0u) ? 1u : 0u) << k;
-            }
-        }
+        if (px0 + 32u <= npix)
+            threshold_word<PB, S, GRAY>(staged ? sa + lane * 32u * PB : pj.prev + (size_t)px0 * PB,
+                                        staged ? sb + lane * 32u * PB : pj.curr + (size_t)px0 * PB, staged, t, m, r);
+        else
+            threshold_word_tail<PB, S, GRAY>(pj.prev + (size_t)px0 * PB, pj.curr + (size_t)px0 * PB, npix - px0, t, m, r);
         pj.mask[w] = m;
         cnt_ones += __popc(m);
         cnt_res += __popc(r);
@@ -195,6 +227,91 @@ __global__ void __launch_bounds__(K1_THREADS) k_threshold(const PairJob* __restr
         for (int i = 0; i < (int)(blockDim.x >> 5); i++) { to += s_o[i]; tr += s_r[i]; }
         if (to) atomicAdd(ones + blockIdx.y, to);
         if (tr) atomicAdd(resid + blockIdx.y, tr);
+    }
+}
+
+// ------------------------------------------------------------------------------------------
+// K1 over a chain of pairs (pairs[t].curr == pairs[t+1].prev, 16 B aligned frames).  k_threshold reads every frame twice, as curr
+// of pair t-1 and as prev of pair t, and only an accident of scheduling lets the second read hit L2.  Here a persistent CTA takes
+// a tile of SW_TILE_PX pixels and sweeps it through the frames prev(0), curr(0), curr(1), ..., curr(P-1): each frame tile is
+// copied once, by cp.async.bulk into a ring of SW_STAGES slots (one mbarrier each), and is compared as curr of pair t-1 and as
+// prev of pair t.  One thread per mask word; the compare is threshold_word, as in k_threshold.
+// Ragged end: the bulk copy of the last tile of a frame is rounded down to 16 B, which still holds every whole 32-pixel word of
+// the tile (a word ends on a multiple of 32 B); the ragged last word of the frame (< 32 px) is read from global memory by
+// threshold_word_tail.  Mask words at or beyond ceil(npix/32) are not written.
+// ------------------------------------------------------------------------------------------
+constexpr int SW_THREADS = 128;
+constexpr uint32_t SW_TILE_PX = 32u * SW_THREADS;     // 4096 px: 4 / 8 / 12 / 24 KB per frame tile at 1 / 2 / 3 / 6 B per pixel
+constexpr int SW_STAGES = 4;                          // frames t and t+1 are read while t+2 and t+3 are in flight
+
+template <int PB, int S, bool GRAY = false>
+__global__ void __launch_bounds__(SW_THREADS) k_threshold_sweep(const PairJob* __restrict__ pairs, uint32_t P, uint32_t npix, int thr,
+                                                                int any_mode, uint32_t* __restrict__ ones, uint32_t* __restrict__ resid) {
+    static_assert(!GRAY || PB == 3 * S, "BGR->gray needs three samples per pixel");
+    constexpr uint32_t SLOT = SW_TILE_PX * PB;
+    constexpr int NWARP = SW_THREADS / 32;
+    extern __shared__ __align__(128) uint8_t ring[];                   // [SW_STAGES][SLOT]
+    __shared__ __align__(8) uint64_t full[SW_STAGES];
+    __shared__ uint32_t s_cnt[2][NWARP][2];                            // per-warp (ones, resid) of the last two frames
+    const uint32_t nwords = (npix + 31u) >> 5;
+    const uint32_t ntiles = (npix + SW_TILE_PX - 1u) / SW_TILE_PX;
+    const uint32_t my_tiles = blockIdx.x < ntiles ? (ntiles - 1u - blockIdx.x) / gridDim.x + 1u : 0u;
+    const uint32_t nfr = P + 1u;                                       // frames of the chain
+    const uint64_t total = (uint64_t)my_tiles * nfr;                   // this CTA's (tile, frame) loads, tile-major
+    const K1Thr t = k1_thr(thr, any_mode);
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < SW_STAGES; s++) mbar_init(&full[s], 1);
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    // load i = (k-th tile of this CTA, frame j) into slot i % SW_STAGES; one thread issues
+    auto issue = [&](uint64_t i) {
+        const uint32_t k = (uint32_t)(i / nfr), j = (uint32_t)(i % nfr);
+        const uint32_t px0 = (blockIdx.x + k * gridDim.x) * SW_TILE_PX;
+        const uint32_t tpx = npix - px0 < SW_TILE_PX ? npix - px0 : SW_TILE_PX;
+        const uint32_t bytes = (tpx * PB) & ~15u;                      // whole 16 B units inside the frame
+        const uint8_t* frame = j == 0 ? pairs[0].prev : pairs[j - 1].curr;
+        uint64_t* bar = &full[i % SW_STAGES];
+        mbar_expect_tx(bar, bytes);                                    // also the one arrival: a 0-byte load completes at once
+        if (bytes) bulk_g2s(ring + (i % SW_STAGES) * SLOT, frame + (size_t)px0 * PB, bytes, bar);
+    };
+    if (threadIdx.x == 0)
+        for (uint64_t i = 0; i < SW_STAGES - 1 && i < total; i++) issue(i);
+
+    uint32_t k = 0, j = 0;                                             // tile and frame of load i
+    for (uint64_t i = 0; i < total; i++) {
+        mbar_wait(&full[i % SW_STAGES], (uint32_t)(i / SW_STAGES) & 1u);
+        if (j > 0) {                                                   // pair j-1: frame j-1 (previous slot) against frame j
+            const PairJob pj = pairs[j - 1];
+            const uint32_t w = (blockIdx.x + k * gridDim.x) * SW_THREADS + threadIdx.x;
+            uint32_t m = 0, r = 0;
+            if (w < nwords) {
+                const uint32_t px0 = w << 5;
+                if (px0 + 32u <= npix)
+                    threshold_word<PB, S, GRAY>(ring + ((i - 1) % SW_STAGES) * SLOT + threadIdx.x * 32u * PB,
+                                                ring + (i % SW_STAGES) * SLOT + threadIdx.x * 32u * PB, true, t, m, r);
+                else
+                    threshold_word_tail<PB, S, GRAY>(pj.prev + (size_t)px0 * PB, pj.curr + (size_t)px0 * PB, npix - px0, t, m, r);
+                pj.mask[w] = m;
+            }
+            const uint32_t co = __reduce_add_sync(0xffffffffu, __popc(m)), cr = __reduce_add_sync(0xffffffffu, __popc(r));
+            if (lane == 0) { s_cnt[i & 1][warp][0] = co; s_cnt[i & 1][warp][1] = cr; }
+        }
+        __syncthreads();                                               // the previous slot has been read by every thread
+        if (threadIdx.x == 0) {
+            if (j > 0) {
+                uint32_t to = 0, tr = 0;
+#pragma unroll
+                for (int q = 0; q < NWARP; q++) { to += s_cnt[i & 1][q][0]; tr += s_cnt[i & 1][q][1]; }
+                if (to) atomicAdd(ones + j - 1, to);
+                if (tr) atomicAdd(resid + j - 1, tr);
+            }
+            if (i + SW_STAGES - 1 < total) { fence_proxy_async(); issue(i + SW_STAGES - 1); }   // into the slot just freed
+        }
+        if (++j == nfr) { j = 0; k++; }
     }
 }
 

@@ -1,6 +1,7 @@
 // rbf_kernels.cu -- hand-written sm_90a kernels of the rational-Bloom hot path.
 //
 //   K1  k_threshold      |Y_prev - Y_curr| > thr  -> packed mask + ones count      (ivc:788-808, ivc:211)
+//       k_threshold_sweep  the same over a chain of pairs, every frame read once
 //   K2  k_insert         insert every set position into the frame's Bloom filter    (ivc:235-237, ivc:99-114)
 //   K3  k_query          Bloom test of ALL n positions -> pass mask                 (ivc:245-253, ivc:116-138)
 //   K3b k_witness        ordered witness = mask bits at passing positions           (ivc:253)
@@ -109,9 +110,30 @@ __device__ __forceinline__ void or_bits128(uint32_t* __restrict__ W, uint64_t bi
 // ------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------
+// K1 over a chain of F >= 2 pairs: persistent CTAs, at most ctas_per_sm per SM, each sweeping the same number of tiles (or one fewer)
+template <int PB, int S, bool GRAY>
+static cudaError_t launch_threshold_sweep_t(const PairJob* d_pairs, int F, uint32_t npix, int thr, int any_mode, uint32_t* d_ones,
+                                            uint32_t* d_resid, int sm_count, int ctas_per_sm, cudaStream_t st) {
+    const int smem = SW_STAGES * (int)SW_TILE_PX * PB;
+    cudaError_t e = cudaFuncSetAttribute(k_threshold_sweep<PB, S, GRAY>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return e;
+    int per_sm = 1;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_threshold_sweep<PB, S, GRAY>, SW_THREADS, (size_t)smem);
+    if (e != cudaSuccess) return e;
+    const int cap = ctas_per_sm > 0 ? ctas_per_sm : 32;
+    if (per_sm > cap) per_sm = cap;
+    if (per_sm < 1) per_sm = 1;
+    const uint32_t ntiles = (npix + SW_TILE_PX - 1u) / SW_TILE_PX;
+    const uint32_t slots = (uint32_t)(sm_count > 0 ? sm_count : 1) * (uint32_t)per_sm;
+    const uint32_t rounds = (ntiles + slots - 1u) / slots;
+    const uint32_t grid = (ntiles + rounds - 1u) / rounds;
+    k_threshold_sweep<PB, S, GRAY><<<grid, SW_THREADS, smem, st>>>(d_pairs, (uint32_t)F, npix, thr, any_mode, d_ones, d_resid);
+    return cudaGetLastError();
+}
+
 template <int PB, int S>
 static cudaError_t launch_threshold_t(const PairJob* d_pairs, int F, uint32_t npix, int thr, int any_mode, uint32_t* d_ones,
-                                      uint32_t* d_resid, int variant, int sm_count, int ctas_per_sm, cudaStream_t st) {
+                                      uint32_t* d_resid, int variant, bool chain, int sm_count, int ctas_per_sm, cudaStream_t st) {
     const uint32_t nwords = (npix + 31u) >> 5;
     constexpr uint32_t TP = TMA_TILE_BYTES / PB;
     if (variant == 1 && npix >= TP && (TP / 32u / (TMA_THREADS / 32)) <= 32u) {
@@ -131,6 +153,7 @@ static cudaError_t launch_threshold_t(const PairJob* d_pairs, int F, uint32_t np
         }
         return cudaGetLastError();
     }
+    if (chain && F >= 2) return launch_threshold_sweep_t<PB, S, false>(d_pairs, F, npix, thr, any_mode, d_ones, d_resid, sm_count, ctas_per_sm, st);
     uint32_t bx = (nwords + 255u) / 256u;
     const uint32_t cap = (uint32_t)(sm_count * (ctas_per_sm > 0 ? ctas_per_sm : 32));
     if ((uint64_t)bx * (uint64_t)F > cap) { bx = (cap + (uint32_t)F - 1u) / (uint32_t)F; if (bx < 1u) bx = 1u; }
@@ -145,7 +168,8 @@ static cudaError_t launch_threshold_t(const PairJob* d_pairs, int F, uint32_t np
 // gray_mode: the mask is taken on cv2.COLOR_BGR2GRAY of the three samples instead of on sample 0 (ivc:792-795)
 template <int PB, int S>
 static cudaError_t launch_threshold_gray_t(const PairJob* d_pairs, int F, uint32_t npix, int thr, int any_mode, uint32_t* d_ones,
-                                           uint32_t* d_resid, int sm_count, int ctas_per_sm, cudaStream_t st) {
+                                           uint32_t* d_resid, bool chain, int sm_count, int ctas_per_sm, cudaStream_t st) {
+    if (chain && F >= 2) return launch_threshold_sweep_t<PB, S, true>(d_pairs, F, npix, thr, any_mode, d_ones, d_resid, sm_count, ctas_per_sm, st);
     const uint32_t nwords = (npix + 31u) >> 5;
     uint32_t bx = (nwords + 255u) / 256u;
     const uint32_t cap = (uint32_t)(sm_count * (ctas_per_sm > 0 ? ctas_per_sm : 32));
@@ -159,19 +183,19 @@ static cudaError_t launch_threshold_gray_t(const PairJob* d_pairs, int F, uint32
 }
 
 cudaError_t launch_threshold(const PairJob* d_pairs, int F, uint32_t npix, int channels, int sample_bytes, int thr_int,
-                             int any_mode, int gray_mode, uint32_t* d_ones, uint32_t* d_resid, int variant, int sm_count,
-                             int ctas_per_sm, cudaStream_t st) {
+                             int any_mode, int gray_mode, uint32_t* d_ones, uint32_t* d_resid, int variant, bool chain,
+                             int sm_count, int ctas_per_sm, cudaStream_t st) {
     if (F <= 0 || npix == 0) return cudaSuccess;
     const int pb = channels * sample_bytes;
     if (gray_mode) {
-        if (pb == 3 && sample_bytes == 1) return launch_threshold_gray_t<3, 1>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, sm_count, ctas_per_sm, st);
-        if (pb == 6 && sample_bytes == 2) return launch_threshold_gray_t<6, 2>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, sm_count, ctas_per_sm, st);
+        if (pb == 3 && sample_bytes == 1) return launch_threshold_gray_t<3, 1>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, sm_count, ctas_per_sm, st);
+        if (pb == 6 && sample_bytes == 2) return launch_threshold_gray_t<6, 2>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, sm_count, ctas_per_sm, st);
         return cudaErrorInvalidValue;
     }
-    if (pb == 3 && sample_bytes == 1) return launch_threshold_t<3, 1>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, variant, sm_count, ctas_per_sm, st);
-    if (pb == 6 && sample_bytes == 2) return launch_threshold_t<6, 2>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, variant, sm_count, ctas_per_sm, st);
-    if (pb == 1 && sample_bytes == 1) return launch_threshold_t<1, 1>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, variant, sm_count, ctas_per_sm, st);
-    if (pb == 2 && sample_bytes == 2) return launch_threshold_t<2, 2>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, variant, sm_count, ctas_per_sm, st);
+    if (pb == 3 && sample_bytes == 1) return launch_threshold_t<3, 1>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, variant, chain, sm_count, ctas_per_sm, st);
+    if (pb == 6 && sample_bytes == 2) return launch_threshold_t<6, 2>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, variant, chain, sm_count, ctas_per_sm, st);
+    if (pb == 1 && sample_bytes == 1) return launch_threshold_t<1, 1>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, variant, chain, sm_count, ctas_per_sm, st);
+    if (pb == 2 && sample_bytes == 2) return launch_threshold_t<2, 2>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, variant, chain, sm_count, ctas_per_sm, st);
     return cudaErrorInvalidValue;
 }
 

@@ -47,9 +47,10 @@ struct GatherJob {
 
 
 // launchers (all asynchronous on `st`); return cudaError_t of the launch
+// chain: the F pairs satisfy pairs[t].curr == pairs[t+1].prev and their frames are 16 B aligned (K1 then reads each frame once)
 cudaError_t launch_threshold(const PairJob* d_pairs, int F, uint32_t npix, int channels, int sample_bytes,
                              int thr_int, int any_mode, int gray_mode, uint32_t* d_ones, uint32_t* d_resid, int variant,
-                             int sm_count, int ctas_per_sm, cudaStream_t st);
+                             bool chain, int sm_count, int ctas_per_sm, cudaStream_t st);
 cudaError_t launch_insert(const FrameJob* d_jobs, int F, uint32_t max_centuries, int variant, int sm_count, cudaStream_t st);
 cudaError_t launch_query(const FrameJob* d_jobs, const uint32_t* d_cent_prefix, int F, uint32_t total_centuries,
                          uint32_t max_l_bits, int variant, int sm_count, int smem_bytes_cap, int tile_warps, cudaStream_t st);
