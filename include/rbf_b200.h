@@ -194,6 +194,25 @@ int rbf_stream_download(rbf_stream* s, uint32_t frame, void* host_out);
 int rbf_median_blur5(rbf_ctx* ctx, const void* plane_in, uint32_t height, uint32_t width, uint32_t sample_bytes, void* plane_out);
 int rbf_stream_median5(rbf_stream* s, uint32_t frame, void* plane_out);   /* channel 0 of a resident frame */
 
+/* ---- SURVEY 8(f) row N4: the zlib entropy stage (fvc:31, ivc:956) coded on the device.  Each input buffer becomes one zlib
+ *     stream (RFC 1950/1951) that zlib.decompress reads; the bytes differ from zlib's own, the decoded data do not.  Layout:
+ *     78 9C | per 64 KiB segment: dynamic-Huffman or stored blocks, BFINAL 0, then 00 00 FF FF (sync flush) | 03 00 | Adler-32
+ *     (big-endian); empty input is 78 9C 03 00 00 00 00 01.  The output is a pure function of the input bytes.
+ * rbf_zlib_bound: worst-case stream size for n input bytes (host scalar, no GPU) */
+uint64_t rbf_zlib_bound(uint64_t n);
+/* the length-limited Huffman code-length builder the kernels use (host scalar, no GPU): lengths[nsym] <= max_bits,
+ * unused symbols 0 and a complete code, except that fewer than two used symbols get exactly two codes of length 1.
+ * nsym 2..288, max_bits 1..15 */
+int rbf_deflate_code_lengths(const uint32_t* freqs, uint32_t nsym, uint32_t max_bits, uint8_t* lengths);
+/* one zlib stream per buffer: srcs[count] (device pointers when srcs_on_device, else host) of lens[count] bytes -> the streams
+ * back to back in out_host; stream i is out_host[out_offsets[i], out_offsets[i+1]).  out_capacity >= sum of rbf_zlib_bound(lens[i])
+ * always suffices; device scratch does not grow with the input (segments are coded in waves). */
+int rbf_zlib_compress_batch(rbf_ctx* ctx, uint32_t count, const void* const* srcs, const uint64_t* lens, int srcs_on_device,
+                            uint8_t* out_host, uint64_t out_capacity, uint64_t* out_offsets /* count+1 */);
+/* N1 + N4: the changed values rbf_stream_gather_changed returns for pairs [0, pairs) of the last encode, gathered and deflated on
+ * the device, one zlib stream per pair (the raw values never cross PCIe); out_offsets[pairs+1] as above */
+int rbf_stream_zlib_changed(rbf_stream* s, uint32_t pairs, uint8_t* out_host, uint64_t out_capacity, uint64_t* out_offsets);
+
 /* ------------------------------------------------------------------ multi-GPU (one process per GPU)
  * frames are sharded across ranks; the per-rank Bloom bit arrays are exchanged with ONE ncclAllGather
  * over NVLink.  NCCL is dlopen'ed (libnccl.so.2); the unique id travels over the caller's own channel. */

@@ -8,6 +8,7 @@ Host code is Python calling hand-written CUDA through a C ABI (include/rbf_b200.
 There is no CPU fallback: importing is cheap, but every entry point needs librbf_b200.so and an H100.
 """
 from . import _cabi
+from . import deflate
 from ._cabi import RbfError
 from .improved_video_compressor import (BloomFilterCompressor, ImprovedVideoCompressor, VideoFrameCompressor)
 from .improved_video_compressor import RationalBloomFilter as IndexRationalBloomFilter
@@ -17,4 +18,4 @@ from .stream import FrameStream, PairResult
 
 __all__ = ["ImprovedVideoCompressor", "VideoFrameCompressor", "BloomFilterCompressor", "IndexRationalBloomFilter",
            "RationalBloomFilter", "StandardBloomFilter", "FixedVideoCompressor", "YUVFrame", "FrameStream",
-           "PairResult", "RbfError"]
+           "PairResult", "RbfError", "deflate"]

@@ -49,6 +49,7 @@ EXPORTS = [
     "rbf_stream_create", "rbf_stream_destroy", "rbf_stream_set_option", "rbf_stream_upload", "rbf_stream_frame_ptr", "rbf_stream_encode",
     "rbf_stream_encode_host", "rbf_stream_fetch", "rbf_stream_fetch_batch", "rbf_stream_decode_verify", "rbf_stream_bitmap_region", "rbf_stream_stage_ms",
     "rbf_stream_gather_changed", "rbf_stream_apply_diff", "rbf_stream_download", "rbf_median_blur5", "rbf_stream_median5",
+    "rbf_zlib_bound", "rbf_deflate_code_lengths", "rbf_zlib_compress_batch", "rbf_stream_zlib_changed",
     "rbf_nccl_unique_id", "rbf_nccl_init", "rbf_nccl_allgather", "rbf_stream_allgather_bitmaps", "rbf_nccl_destroy",
     "rbf_peer_export", "rbf_peer_open", "rbf_peer_close", "rbf_peer_gather_init", "rbf_peer_gather_half", "rbf_peer_gather_shutdown",
 ]
@@ -119,6 +120,11 @@ def _sig(L):
     L.rbf_stream_download.argtypes = [vp, u32, vp]
     L.rbf_median_blur5.argtypes = [vp, vp, u32, u32, u32, vp]
     L.rbf_stream_median5.argtypes = [vp, u32, vp]
+    L.rbf_zlib_bound.argtypes = [u64]
+    L.rbf_zlib_bound.restype = u64
+    L.rbf_deflate_code_lengths.argtypes = [vp, u32, u32, vp]
+    L.rbf_zlib_compress_batch.argtypes = [vp, u32, vp, vp, i32, vp, u64, vp]
+    L.rbf_stream_zlib_changed.argtypes = [vp, u32, vp, u64, vp]
     L.rbf_nccl_unique_id.argtypes = [vp]
     L.rbf_nccl_init.argtypes = [vp, vp, i32, i32]
     L.rbf_nccl_allgather.argtypes = [vp, vp, vp, u64]
@@ -202,3 +208,16 @@ def optimal_params(n: int, ones: int):
     p, k, l = C.c_double(), C.c_double(), C.c_uint64()
     coded = lib().rbf_optimal_params(int(n), int(ones), C.byref(p), C.byref(k), C.byref(l))
     return bool(coded), p.value, k.value, int(l.value)
+
+
+def zlib_bound(n: int) -> int:
+    """Worst-case size of the zlib stream the device coder writes for n input bytes."""
+    return int(lib().rbf_zlib_bound(int(n)))
+
+
+def deflate_code_lengths(freqs, max_bits: int) -> np.ndarray:
+    """The kernels' length-limited Huffman code lengths for a frequency vector (host scalar helper)."""
+    f = np.ascontiguousarray(np.asarray(freqs, dtype=np.uint32))
+    out = np.zeros(f.size, dtype=np.uint8)
+    check(lib().rbf_deflate_code_lengths(ptr(f), f.size, int(max_bits), ptr(out)))
+    return out

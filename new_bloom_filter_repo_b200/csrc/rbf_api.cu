@@ -1264,6 +1264,154 @@ extern "C" int rbf_stream_median5(rbf_stream* s, uint32_t frame, void* plane_out
 }
 
 // ------------------------------------------------------------------------------------------
+// N4: zlib streams coded on the device (layout: rbf_deflate.cuh)
+// ------------------------------------------------------------------------------------------
+extern "C" uint64_t rbf_zlib_bound(uint64_t n) {
+    if (n == 0) return 8;
+    const uint64_t full = (n - 1) / kDeflateSeg, last = n - full * kDeflateSeg;
+    return 2 + full * deflate_seg_bound(kDeflateSeg) + deflate_seg_bound((uint32_t)last) + 6;
+}
+
+extern "C" int rbf_deflate_code_lengths(const uint32_t* freqs, uint32_t nsym, uint32_t max_bits, uint8_t* lengths) {
+    if (!freqs || !lengths) return set_err(nullptr, RBF_ERR_INVALID, "rbf_deflate_code_lengths: NULL");
+    if (deflate_code_lengths_host(freqs, nsym, max_bits, lengths))
+        return set_err(nullptr, RBF_ERR_INVALID, "rbf_deflate_code_lengths: nsym %u / max_bits %u not codable", nsym, max_bits);
+    return RBF_OK;
+}
+
+// Segments are coded in waves of at most 2 per SM, so scratch is bounded whatever the input size; each wave's streams are
+// joined on the device and copied to out_host with one copy.
+static int zlib_batch(rbf_ctx* c, uint32_t count, const void* const* srcs, const uint64_t* lens, bool on_device, uint8_t* out_host,
+                      uint64_t capacity, uint64_t* offsets) {
+    CK(c, cudaSetDevice(c->device));
+    offsets[0] = 0;
+    if (count == 0) return RBF_OK;
+    for (uint32_t b = 0; b < count; b++)
+        if (lens[b] && !srcs[b]) return set_err(c, RBF_ERR_INVALID, "zlib: buffer %u is NULL", b);
+    const uint32_t W = 2u * (uint32_t)(c->sm_count > 0 ? c->sm_count : 1);
+    const size_t region = align_up(deflate_seg_bound(kDeflateSeg), 16), stage_cap = (size_t)W * (region + 8);
+    void *d_in = nullptr, *d_res, *d_out, *d_stage, *d_segs, *d_copies, *d_small;
+    int rc;
+    if ((rc = scratch_get(c, 14, (size_t)W * kDeflateSeg * 4, &d_res)) || (rc = scratch_get(c, 15, (size_t)W * region, &d_out)) ||
+        (rc = scratch_get(c, 16, stage_cap, &d_stage)) || (rc = scratch_get(c, 17, (size_t)W * sizeof(DeflateSeg), &d_segs)) ||
+        (rc = scratch_get(c, 18, (size_t)W * sizeof(DeflateCopy), &d_copies)) || (rc = scratch_get(c, 19, (size_t)W * 12 + 64, &d_small)) ||
+        (!on_device && (rc = scratch_get(c, 20, (size_t)W * kDeflateSeg, &d_in))))
+        return rc;
+    uint32_t* d_sizes = (uint32_t*)d_small;
+    uint32_t* d_adler = d_sizes + W;
+    uint32_t* d_err = d_adler + 2 * W;
+    struct Ref { uint32_t buf; uint64_t off; uint32_t len; bool first, last; };
+    std::vector<Ref> refs;
+    std::vector<DeflateSeg> segs;
+    std::vector<DeflateCopy> copies;
+    std::vector<uint32_t> h_small(3 * (size_t)W + 1);
+    uint32_t b = 0;
+    uint64_t k = 0, pos = 0;
+    uint32_t s1 = 1, s2 = 0;                                              // Adler-32 of the buffer being written
+    while (b < count) {
+        refs.clear(); segs.clear(); copies.clear();
+        while (refs.size() < W && b < count) {
+            const uint64_t nseg = lens[b] ? (lens[b] + kDeflateSeg - 1) / kDeflateSeg : 1, off = k * kDeflateSeg;
+            const uint64_t left = lens[b] - (lens[b] ? off : 0);
+            refs.push_back({b, off, (uint32_t)(left < kDeflateSeg ? left : kDeflateSeg), k == 0, k + 1 == nseg});
+            if (++k == nseg) { b++; k = 0; }
+        }
+        const uint32_t n = (uint32_t)refs.size();
+        for (uint32_t i = 0; i < n; i++) {
+            const Ref& r = refs[i];
+            DeflateSeg sg;
+            sg.src = on_device ? (const uint8_t*)srcs[r.buf] + r.off : (const uint8_t*)d_in + (size_t)i * kDeflateSeg;
+            sg.out = (uint8_t*)d_out + (size_t)i * region;
+            sg.len = r.len;
+            sg.cap = (uint32_t)region;
+            segs.push_back(sg);
+            if (!on_device && r.len && (i == 0 || refs[i - 1].buf != r.buf)) {   // the wave's part of one buffer is contiguous
+                uint64_t bytes = 0;
+                for (uint32_t j = i; j < n && refs[j].buf == r.buf; j++) bytes += refs[j].len;
+                CK(c, cudaMemcpyAsync((uint8_t*)d_in + (size_t)i * kDeflateSeg, (const uint8_t*)srcs[r.buf] + r.off, bytes,
+                                      cudaMemcpyHostToDevice, c->st));
+                c->h2d += (int64_t)bytes;
+            }
+        }
+        CK(c, cudaMemsetAsync(d_err, 0, 4, c->st));
+        CK(c, cudaMemcpyAsync(d_segs, segs.data(), sizeof(DeflateSeg) * n, cudaMemcpyHostToDevice, c->st));
+        LAUNCH(c, launch_deflate_segments((const DeflateSeg*)d_segs, (int)n, (uint32_t*)d_res, d_sizes, d_adler, d_err, c->st));
+        CK(c, cudaMemcpyAsync(h_small.data(), d_small, (3 * (size_t)W + 1) * 4, cudaMemcpyDeviceToHost, c->st));
+        CK(c, cudaStreamSynchronize(c->st));
+        if (h_small[3 * (size_t)W]) return set_err(c, RBF_ERR_STATE, "zlib: a coded segment overran its region (flags %u)", h_small[3 * (size_t)W]);
+        const uint64_t wave_start = pos;
+        for (uint32_t i = 0; i < n; i++) {
+            const Ref& r = refs[i];
+            const uint32_t size = h_small[i];
+            if (r.first) { offsets[r.buf] = pos; pos += 2; s1 = 1; s2 = 0; }
+            s2 = (uint32_t)((s2 + (uint64_t)r.len * s1 + h_small[W + 2 * i + 1]) % 65521u);
+            s1 = (uint32_t)((s1 + h_small[W + 2 * i]) % 65521u);
+            DeflateCopy cp;
+            cp.src = (const uint8_t*)d_out + (size_t)i * region;
+            cp.dst = pos - wave_start;
+            cp.len = size;
+            cp.flags = (r.first ? 1u : 0u) | (r.last ? 2u : 0u);
+            cp.adler = (s2 << 16) | s1;
+            cp.pad = 0;
+            copies.push_back(cp);
+            pos += size;
+            if (r.last) { pos += 6; offsets[r.buf + 1] = pos; }
+        }
+        if (pos > capacity)
+            return set_err(c, RBF_ERR_INVALID, "zlib: output buffer too small (%llu < %llu so far)", (unsigned long long)capacity,
+                           (unsigned long long)pos);
+        CK(c, cudaMemcpyAsync(d_copies, copies.data(), sizeof(DeflateCopy) * n, cudaMemcpyHostToDevice, c->st));
+        LAUNCH(c, launch_deflate_concat((const DeflateCopy*)d_copies, (int)n, (uint8_t*)d_stage, stage_cap, d_err, c->st));
+        CK(c, cudaMemcpyAsync(out_host + wave_start, d_stage, (size_t)(pos - wave_start), cudaMemcpyDeviceToHost, c->st));
+        CK(c, cudaMemcpyAsync(h_small.data() + 3 * (size_t)W, d_err, 4, cudaMemcpyDeviceToHost, c->st));
+        c->d2h += (int64_t)(pos - wave_start);
+        CK(c, cudaStreamSynchronize(c->st));
+        if (h_small[3 * (size_t)W]) return set_err(c, RBF_ERR_STATE, "zlib: joined streams overran the staging buffer");
+    }
+    return RBF_OK;
+}
+
+extern "C" int rbf_zlib_compress_batch(rbf_ctx* c, uint32_t count, const void* const* srcs, const uint64_t* lens, int srcs_on_device,
+                                       uint8_t* out_host, uint64_t out_capacity, uint64_t* out_offsets) {
+    if (!c || !out_offsets || (count && (!srcs || !lens || !out_host))) return set_err(c, RBF_ERR_INVALID, "rbf_zlib_compress_batch: NULL");
+    return zlib_batch(c, count, srcs, lens, srcs_on_device != 0, out_host, out_capacity, out_offsets);
+}
+
+extern "C" int rbf_stream_zlib_changed(rbf_stream* s, uint32_t pairs, uint8_t* out_host, uint64_t out_capacity, uint64_t* out_offsets) {
+    if (!s || !out_host || !out_offsets) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_zlib_changed: NULL");
+    rbf_ctx* c = s->c;
+    if (pairs == 0 || pairs > s->last_pairs) return set_err(c, RBF_ERR_INVALID, "only %u pairs were encoded", s->last_pairs);
+    CK(c, cudaSetDevice(c->device));
+    const uint64_t pb = (uint64_t)s->C * s->S;
+    std::vector<uint64_t> voff(pairs + 1);
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < pairs; i++) { voff[i] = total; total += s->last_infos[i].ones * pb; }
+    voff[pairs] = total;
+    void *d_vals, *d_jobs, *d_gcnt;
+    int rc;
+    if ((rc = scratch_get(c, 8, (size_t)total + 256, &d_vals)) || (rc = scratch_get(c, 9, sizeof(GatherJob) * pairs, &d_jobs)) ||
+        (rc = scratch_get(c, 13, 4 * (size_t)pairs * gather_chunks((uint32_t)s->npix) + 64, &d_gcnt)))
+        return rc;
+    std::vector<GatherJob> jobs(pairs);
+    std::vector<const void*> srcs(pairs);
+    std::vector<uint64_t> lens(pairs);
+    for (uint32_t i = 0; i < pairs; i++) {
+        jobs[i].mask = s->d_mask + (size_t)i * s->mask_stride_w;
+        jobs[i].frame = s->h_pairs[i].curr;
+        jobs[i].values = (uint8_t*)d_vals + voff[i];
+        jobs[i].out_frame = nullptr;
+        jobs[i].npix = (uint32_t)s->npix;
+        jobs[i].pix_bytes = (uint32_t)pb;
+        srcs[i] = jobs[i].values;
+        lens[i] = voff[i + 1] - voff[i];
+    }
+    CK(c, cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(GatherJob) * pairs, cudaMemcpyHostToDevice, c->st));
+    LAUNCH(c, launch_gather_scatter((const GatherJob*)d_jobs, (int)pairs, 0, (uint32_t)s->npix, (uint32_t)pb, (uint32_t*)d_gcnt, nullptr, c->st));
+    c->launches++;
+    return zlib_batch(c, pairs, srcs.data(), lens.data(), true, out_host, out_capacity, out_offsets);   // same stream: after the gather
+}
+
+// ------------------------------------------------------------------------------------------
 // NCCL (dlopen'ed so that single-GPU use needs no NCCL at all)
 // ------------------------------------------------------------------------------------------
 typedef struct { char internal[128]; } nccl_uid;

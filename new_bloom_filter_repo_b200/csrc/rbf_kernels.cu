@@ -6,13 +6,14 @@
 //   K3  k_query          Bloom test of ALL n positions -> pass mask                 (ivc:245-253, ivc:116-138)
 //   K3b k_witness        ordered witness = mask bits at passing positions           (ivc:253)
 //   K4b k_expand         decode: out[i] = witness[rank(i)] for passing i            (ivc:299-304)
+//   N4  k_deflate_segments / k_deflate_concat   zlib streams of host or device buffers (rbf_deflate.cuh)
 //
 // The Bloom bit array of the frame being queried is staged into shared memory with
 // cp.async.bulk (TMA bulk copy, mbarrier complete_tx); whatever exceeds the 227 KB of a
 // CTA is probed through L2.  Integer hashing / bit tests only: no tensor cores.
 //
 // One translation unit: this file holds the PTX helpers and the launchers; the kernels live in
-// rbf_k1_threshold.cuh, rbf_k2_insert.cuh, rbf_k3_query.cuh, rbf_k3b_witness.cuh and rbf_aux_kernels.cuh.
+// rbf_k1_threshold.cuh, rbf_k2_insert.cuh, rbf_k3_query.cuh, rbf_k3b_witness.cuh, rbf_aux_kernels.cuh and rbf_deflate.cuh.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -106,6 +107,7 @@ __device__ __forceinline__ void or_bits128(uint32_t* __restrict__ W, uint64_t bi
 #include "rbf_k3_query.cuh"
 #include "rbf_k3b_witness.cuh"
 #include "rbf_aux_kernels.cuh"
+#include "rbf_deflate.cuh"
 
 // ------------------------------------------------------------------------------------------
 // launchers
@@ -428,6 +430,25 @@ cudaError_t launch_push_slots(const uint32_t* d_bits, size_t stride_w, uint32_t 
 cudaError_t launch_peer_wait(const uint32_t* d_flags, int nranks, uint32_t seq, long long timeout_cycles, uint32_t* d_err, cudaStream_t st) {
     k_peer_wait<<<1, 32, 0, st>>>(d_flags, nranks, seq, timeout_cycles, d_err);
     return cudaGetLastError();
+}
+
+// N4: one CTA per segment; d_res: kDeflateSeg uint32 per segment of the launch
+cudaError_t launch_deflate_segments(const DeflateSeg* d_segs, int count, uint32_t* d_res, uint32_t* d_sizes, uint32_t* d_adler,
+                                    uint32_t* d_err, cudaStream_t st) {
+    if (count <= 0) return cudaSuccess;
+    cudaError_t e = cudaFuncSetAttribute(k_deflate_segments, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDzBytes);
+    if (e != cudaSuccess) return e;
+    k_deflate_segments<<<count, kDeflateThreads, kDzBytes, st>>>(d_segs, d_res, d_sizes, d_adler, d_err);
+    return cudaGetLastError();
+}
+cudaError_t launch_deflate_concat(const DeflateCopy* d_jobs, int count, uint8_t* d_dst, uint64_t cap, uint32_t* d_err, cudaStream_t st) {
+    if (count <= 0) return cudaSuccess;
+    k_deflate_concat<<<count, 256, 0, st>>>(d_jobs, d_dst, cap, d_err);
+    return cudaGetLastError();
+}
+int deflate_code_lengths_host(const uint32_t* freqs, uint32_t nsym, uint32_t max_bits, uint8_t* lengths) {
+    HuffScratch S;
+    return deflate_code_lengths(freqs, nsym, max_bits, lengths, &S);
 }
 
 }  // namespace rbf

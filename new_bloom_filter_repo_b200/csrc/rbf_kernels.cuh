@@ -46,6 +46,26 @@ struct GatherJob {
 };
 
 
+// N4 deflate (rbf_deflate.cuh): one segment of at most 64 KiB per CTA, and the join of coded segments into zlib streams
+static constexpr uint32_t kDeflateSeg = 65536;         // segment size (bytes); the layout is pinned in rbf_deflate.cuh
+// worst-case output of one segment of n bytes (0 < n <= kDeflateSeg): stored blocks plus the sync flush
+__host__ __device__ __forceinline__ uint32_t deflate_seg_bound(uint32_t n) { return n == 0 ? 0u : n + 5u * (n > 65535u ? 2u : 1u) + 5u; }
+struct DeflateSeg {
+    const uint8_t* src;   // segment bytes (device)
+    uint8_t* out;         // output region (16 B aligned)
+    uint32_t len;         // 0..kDeflateSeg
+    uint32_t cap;         // region bytes
+};
+struct DeflateCopy {
+    const uint8_t* src;   // a segment's coded bytes
+    uint64_t dst;         // byte offset of those bytes in the joined range
+    uint32_t len;
+    uint32_t flags;       // 1: the zlib header goes in front (dst - 2); 2: the trailer goes behind (03 00 + adler)
+    uint32_t adler;       // Adler-32 of the whole stream (flags & 2)
+    uint32_t pad;
+};
+
+
 // launchers (all asynchronous on `st`); return cudaError_t of the launch
 // chain: the F pairs satisfy pairs[t].curr == pairs[t+1].prev and their frames are 16 B aligned (K1 then reads each frame once)
 cudaError_t launch_threshold(const PairJob* d_pairs, int F, uint32_t npix, int channels, int sample_bytes,
@@ -82,6 +102,11 @@ cudaError_t launch_hash_debug(const uint32_t* d_items, uint32_t count, uint64_t 
 cudaError_t launch_push_slots(const uint32_t* d_bits, size_t stride_w, uint32_t slot_w, uint32_t pairs, uint32_t* const* recv,
                               uint32_t* const* flags, int nranks, int rank, size_t dst_off_w, uint32_t seq, int sm_count, cudaStream_t st);
 cudaError_t launch_peer_wait(const uint32_t* d_flags, int nranks, uint32_t seq, long long timeout_cycles, uint32_t* d_err, cudaStream_t st);
+
+cudaError_t launch_deflate_segments(const DeflateSeg* d_segs, int count, uint32_t* d_res, uint32_t* d_sizes, uint32_t* d_adler,
+                                    uint32_t* d_err, cudaStream_t st);
+cudaError_t launch_deflate_concat(const DeflateCopy* d_jobs, int count, uint8_t* d_dst, uint64_t cap, uint32_t* d_err, cudaStream_t st);
+int deflate_code_lengths_host(const uint32_t* freqs, uint32_t nsym, uint32_t max_bits, uint8_t* lengths);
 
 int query_max_smem_bytes();
 

@@ -57,10 +57,26 @@ class YUVFrame:
 _DTYPES = {1: np.uint8, 2: np.uint16}
 
 
-def _put_blob(parts: List[bytes], raw: bytes) -> None:
-    z = zlib.compress(raw, 9)
-    parts.append(struct.pack("<I", len(z)))
-    parts.append(z)
+_PLANES = ("y_plane", "u_plane", "v_plane")
+
+
+def keyframe_raws(frame) -> List[bytes]:
+    """The buffers a keyframe payload compresses: the frame, then (YUV frames) the Y, U and V planes."""
+    info = getattr(frame, "yuv_info", None)
+    return [frame.tobytes()] + ([info[name].tobytes() for name in _PLANES] if info is not None else [])
+
+
+def assemble_keyframe(frame, blobs: List[bytes]) -> bytes:
+    """The keyframe byte layout around already compressed blobs (one per keyframe_raws(frame) entry, any zlib stream)."""
+    info = getattr(frame, "yuv_info", None)
+    parts: List[bytes] = [struct.pack("<III", frame.shape[0], frame.shape[1], frame.dtype.itemsize),
+                          struct.pack("<I", len(blobs[0])), blobs[0], struct.pack("<B", 1 if info is not None else 0)]
+    if info is not None:
+        fmt = info.get("format", "YUV444").encode("utf-8")
+        parts += [struct.pack("<H", len(fmt)), fmt]
+        for zi, name in zip(blobs[1:], _PLANES):
+            parts += [struct.pack("<I", len(zi)), zi, struct.pack("<II", *info[name].shape)]
+    return b"".join(parts)
 
 
 class FixedVideoCompressor:
@@ -71,38 +87,13 @@ class FixedVideoCompressor:
         self.verbose = verbose
 
     def compress_frame(self, frame) -> bytes:                                    # fvc:27-74
-        parts: List[bytes] = [struct.pack("<III", frame.shape[0], frame.shape[1], frame.dtype.itemsize)]
-        _put_blob(parts, frame.tobytes())
-        info = getattr(frame, "yuv_info", None)
-        parts.append(struct.pack("<B", 1 if info is not None else 0))
-        if info is not None:
-            fmt = info.get("format", "YUV444").encode("utf-8")
-            parts.append(struct.pack("<H", len(fmt)))
-            parts.append(fmt)
-            for name in ("y_plane", "u_plane", "v_plane"):
-                plane = info[name]
-                _put_blob(parts, plane.tobytes())
-                parts.append(struct.pack("<II", *plane.shape))
-        return b"".join(parts)
+        return assemble_keyframe(frame, [zlib.compress(r, 9) for r in keyframe_raws(frame)])
 
     def compress_frame_async(self, frame, pool):
         """compress_frame with the (up to four) zlib level-9 blobs as separate jobs of `pool`; returns a callable that assembles
         exactly the bytes compress_frame(frame) returns.  The keyframe of a GOP is the longest serial piece of compress_video."""
-        info = getattr(frame, "yuv_info", None)
-        raws = [frame.tobytes()] + ([info[name].tobytes() for name in ("y_plane", "u_plane", "v_plane")] if info is not None else [])
-        futs = [pool.submit(zlib.compress, r, 9) for r in raws]
-
-        def assemble() -> bytes:
-            z = [f.result() for f in futs]
-            parts: List[bytes] = [struct.pack("<III", frame.shape[0], frame.shape[1], frame.dtype.itemsize),
-                                  struct.pack("<I", len(z[0])), z[0], struct.pack("<B", 1 if info is not None else 0)]
-            if info is not None:
-                fmt = info.get("format", "YUV444").encode("utf-8")
-                parts += [struct.pack("<H", len(fmt)), fmt]
-                for zi, name in zip(z[1:], ("y_plane", "u_plane", "v_plane")):
-                    parts += [struct.pack("<I", len(zi)), zi, struct.pack("<II", *info[name].shape)]
-            return b"".join(parts)
-        return assemble
+        futs = [pool.submit(zlib.compress, r, 9) for r in keyframe_raws(frame)]
+        return lambda: assemble_keyframe(frame, [f.result() for f in futs])
 
     def decompress_frame(self, data: bytes):                                     # fvc:76-181
         h, w, isz = struct.unpack_from("<III", data, 0)

@@ -30,8 +30,8 @@ from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 
-from . import _cabi
-from .fixed_video_compressor import FixedVideoCompressor, YUVFrame
+from . import _cabi, deflate
+from .fixed_video_compressor import FixedVideoCompressor, YUVFrame, assemble_keyframe, keyframe_raws
 from .rational_bloom_filter import _DeviceFilter
 from .stream import FrameStream
 
@@ -358,6 +358,10 @@ class ImprovedVideoCompressor:
                   unflagged pixels changed (chroma-only or sub-threshold changes) falls back to a keyframe.
     The entropy stage (zlib level 9, ivc:956 / fvc:31) stays on the CPU but runs in a thread pool (`num_threads`; zlib
     releases the GIL), and a group of `batch_size` inter frames costs ONE encode call and ONE batched device->host copy.
+    `entropy_coder`:
+      "zlib"  (default) zlib level 9 on the CPU: keyframe_interval=1 writes exactly the reference's bytes;
+      "gpu"   every zlib stream of the payloads (keyframe blobs, changed values, raw-passthrough masks) is coded on the GPU
+              (deflate.py): other compressed bytes, the same decoded data, read by the unchanged decoders.
     """
 
     def __init__(self, noise_tolerance: float = 10.0, keyframe_interval: int = 30, min_diff_threshold: float = 3.0,
@@ -375,24 +379,34 @@ class ImprovedVideoCompressor:
         self.compressor = FixedVideoCompressor(verbose=verbose)                    # ivc:356
         self.inter_frame_mode = "lossless"
         self.inter_frame_threshold = 0.0
+        self.entropy_coder = "zlib"
         _cabi.ctx()                                                                 # fail now if there is no H100
 
     # ------------------------------------------------------------------ encode
     @staticmethod
+    def _raw_mask_bits(shape, mask_row) -> bytes:
+        """Passthrough branch (ivc:215-225): the mask itself in np.packbits order."""
+        n = shape[0] * shape[1]
+        return np.packbits(np.unpackbits(mask_row, bitorder="little")[:n]).tobytes()
+
+    @staticmethod
     def _inter_payload(shape, itemsize, ch, r, bm_row, wt_row, mask_row, values) -> bytes:
         """Assemble one inter-frame payload (runs in a worker thread; the zlib calls release the GIL)."""
         vz = zlib.compress(values.tobytes(), 9)
+        rz = zlib.compress(ImprovedVideoCompressor._raw_mask_bits(shape, mask_row), 9) if r.raw else None
+        return ImprovedVideoCompressor._inter_layout(shape, itemsize, ch, r, bm_row, wt_row, rz, vz, values.size)
+
+    @staticmethod
+    def _inter_layout(shape, itemsize, ch, r, bm_row, wt_row, rz, vz, vcount) -> bytes:
+        """The inter-frame byte layout around the compressed raw mask `rz` (raw pairs only) and changed values `vz`."""
         hdr = _INTER_TAG + struct.pack("<IIIBB", shape[0], shape[1], itemsize, ch, 1 if r.raw else 0)
         body = struct.pack("<dIIQ", r.k, r.l, r.wlen, r.ones)
-        if r.raw:                                              # passthrough branch (ivc:215-225): the mask itself, np.packbits order
-            n = shape[0] * shape[1]
-            raw_bits = np.packbits(np.unpackbits(mask_row, bitorder="little")[:n]).tobytes()
-            rz = zlib.compress(raw_bits, 9)
+        if r.raw:
             body += struct.pack("<I", len(rz)) + rz + struct.pack("<I", 0)
         else:
             nb, nw = (r.l + 7) // 8, (r.wlen + 7) // 8
             body += struct.pack("<I", nb) + bm_row[:nb].tobytes() + struct.pack("<I", nw) + wt_row[:nw].tobytes()
-        body += struct.pack("<II", len(vz), values.size) + vz
+        body += struct.pack("<II", len(vz), vcount) + vz
         return hdr + body
 
     def _encode_inter_frames(self, datas: List[np.ndarray], inter: List[int], pool) -> Dict[int, object]:
@@ -412,9 +426,12 @@ class ImprovedVideoCompressor:
                 slot = {f: s for s, f in enumerate(need)}
                 st.upload(np.stack([datas[f] for f in need]))
                 res = st.encode([slot[i - 1] for i in idxs], [slot[i] for i in idxs], float(self.inter_frame_threshold))
-                gathered = st.gather_changed(len(idxs))            # N1: changed values of every pair, one launch, one copy
                 any_raw = any(r.raw for r in res)
                 bms, wts, masks = st.fetch_batch(0, len(idxs), want_masks=any_raw)   # one D2H per kind, one sync per group
+                if self.entropy_coder == "gpu":
+                    self._gpu_inter_payloads(st, shape, dtype.itemsize, ch, idxs, res, bms, wts, masks, out, pool)
+                    continue
+                gathered = st.gather_changed(len(idxs))            # N1: changed values of every pair, one launch, one copy
                 for j, i in enumerate(idxs):
                     r = res[j]
                     if r.resid and self.inter_frame_mode != "lossless":
@@ -426,7 +443,30 @@ class ImprovedVideoCompressor:
             st.close()
         return out
 
+    def _gpu_inter_payloads(self, st, shape, itemsize, ch, idxs, res, bms, wts, masks, out, pool) -> None:
+        """entropy_coder "gpu": changed values deflated where they were gathered (N1 + N4), raw masks in one batch."""
+        vzs = st.zlib_changed(len(idxs))
+        voffs = st.changed_offsets(len(idxs))
+        keep = [j for j, i in enumerate(idxs) if not (res[j].resid and self.inter_frame_mode != "lossless")]
+        raw_js = [j for j in keep if res[j].raw]
+        rzs = dict(zip(raw_js, deflate.compress_many([self._raw_mask_bits(shape, masks[j]) for j in raw_js])))
+        for j, i in enumerate(idxs):
+            if j not in keep:
+                out[i] = None                                      # not exactly representable: keyframe instead
+                continue
+            vcount = int(voffs[j + 1] - voffs[j]) // itemsize
+            out[i] = pool.submit(self._inter_layout, shape, itemsize, ch, res[j], bms[j], wts[j], rzs.get(j), vzs[j], vcount)
+
+    def _keyframe_job(self, frame, pool):
+        """Callable returning the keyframe payload of `frame`: zlib level 9 in the pool, or coded on the GPU now."""
+        if self.entropy_coder == "gpu":
+            payload = assemble_keyframe(frame, deflate.compress_many(keyframe_raws(frame)))
+            return lambda: payload
+        return self.compressor.compress_frame_async(frame, pool)
+
     def compress_video(self, frames: List[np.ndarray], output_path: str = None, input_color_space: str = "BGR") -> Dict:
+        if self.entropy_coder not in ("zlib", "gpu"):
+            raise ValueError(f"entropy_coder must be 'zlib' or 'gpu', not {self.entropy_coder!r}")
         if not frames:
             raise ValueError("No frames provided for compression")                 # ivc:372-373
         start_time = time.time()
@@ -447,13 +487,13 @@ class ImprovedVideoCompressor:
         with ThreadPoolExecutor(self.num_threads) as pool:
             # keyframes (zlib level 9 of whole frames, fvc:31) start in the pool first; the GPU encodes the groups meanwhile
             inter_set = set(inter)
-            key_jobs = {i: self.compressor.compress_frame_async(frames[i], pool) for i in range(len(frames)) if i not in inter_set}
+            key_jobs = {i: self._keyframe_job(frames[i], pool) for i in range(len(frames)) if i not in inter_set}
             payloads = self._encode_inter_frames(datas, inter, pool)
             for i, f in enumerate(frames):
                 fut = payloads.get(i)
                 if fut is None:
                     kj = key_jobs.get(i)
-                    pl = kj() if kj is not None else self.compressor.compress_frame(f)
+                    pl = (kj if kj is not None else self._keyframe_job(f, pool))()
                     keyframes += 1
                 else:
                     pl = fut.result()

@@ -146,6 +146,23 @@ class FrameStream:
             _cabi.check(_cabi.lib().rbf_stream_gather_changed(self._h, n, _cabi.ptr(buf), buf.size, _cabi.ptr(offs)), _cabi.ctx())
         return [buf[int(offs[i]):int(offs[i + 1])].view(self.dtype) for i in range(n)]
 
+    def changed_offsets(self, pairs: Optional[int] = None) -> np.ndarray:
+        """Byte offsets [pairs+1] of every encoded pair's changed values (what gather_changed returns), without the values."""
+        n = self.pairs if pairs is None else int(pairs)
+        offs = np.zeros(n + 1, dtype=np.uint64)
+        _cabi.check(_cabi.lib().rbf_stream_gather_changed(self._h, n, None, 0, _cabi.ptr(offs)), _cabi.ctx())
+        return offs
+
+    def zlib_changed(self, pairs: Optional[int] = None) -> List[bytes]:
+        """Per encoded pair: a zlib stream of what gather_changed returns, gathered and deflated on the GPU."""
+        n = self.pairs if pairs is None else int(pairs)
+        vo = self.changed_offsets(n)
+        cap = sum(_cabi.zlib_bound(int(vo[i + 1] - vo[i])) for i in range(n))
+        out = np.empty(cap, dtype=np.uint8)
+        offs = np.zeros(n + 1, dtype=np.uint64)
+        _cabi.check(_cabi.lib().rbf_stream_zlib_changed(self._h, n, _cabi.ptr(out), cap, _cabi.ptr(offs)), _cabi.ctx())
+        return [out[int(offs[i]):int(offs[i + 1])].tobytes() for i in range(n)]
+
     def apply_diff(self, base_frame: int, out_frame: int, mask: np.ndarray, values: np.ndarray) -> int:
         """store[out_frame] = store[base_frame] with masked pixels replaced by `values` (ivc:849-909); returns pixels applied."""
         mk = np.packbits(np.ascontiguousarray(mask, dtype=np.uint8).reshape(-1), bitorder="little")

@@ -13,9 +13,10 @@ import new_bloom_filter_repo_b200 as pkg  # noqa: E402
 from tests.util import synth_stream  # noqa: E402
 
 
-def run(h, w, nfr, threads, mode):
+def run(h, w, nfr, threads, mode, coder="zlib"):
     frames = [f for f in synth_stream(h, w, nfr, 2, [0.01, 0.05, 0.15, 0.30])]
     comp = pkg.ImprovedVideoCompressor(keyframe_interval=30, num_threads=threads)
+    comp.entropy_coder = coder
     comp.inter_frame_mode = mode
     comp.inter_frame_threshold = 3.0
     comp.compress_video(list(frames[:4]), input_color_space="YUV")          # warm-up (context, streams, zlib)
@@ -25,7 +26,8 @@ def run(h, w, nfr, threads, mode):
     dec = comp.decompress_video(compressed_frames=comp._last_compressed_frames)
     t2 = time.perf_counter()
     ok = comp.verify_lossless(frames, dec)["lossless"]
-    return {"config": "%dx%d YUV444 x %d frames, keyframe_interval=30, inter_frame_mode=%s" % (w, h, nfr, mode), "zlib_threads": threads or "default(%d)" % comp.num_threads,
+    return {"config": "%dx%d YUV444 x %d frames, keyframe_interval=30, inter_frame_mode=%s" % (w, h, nfr, mode), "entropy_coder": coder,
+            "zlib_threads": threads or "default(%d)" % comp.num_threads,
             "compress_fps": nfr / (t1 - t0), "decompress_fps": nfr / (t2 - t1), "keyframes": stats["keyframes"], "ratio": stats["compression_ratio"],
             "lossless": bool(ok)}
 
@@ -35,9 +37,9 @@ if __name__ == "__main__":
     faulthandler.dump_traceback_later(120, repeat=True)          # a stuck run shows where
     sizes = ((1080, 1920), (2160, 3840)) if "--4k" in sys.argv else ((1080, 1920),)
     for (h, w) in sizes:
-        for threads in (1, None):
+        for coder, threads in (("zlib", 1), ("zlib", None), ("gpu", None)):
             for mode in ("lossless", "reference"):
                 t0 = time.perf_counter()
-                line = run(h, w, 30, threads, mode)
+                line = run(h, w, 30, threads, mode, coder)
                 line["wall_s_incl_synthesis_and_warmup"] = time.perf_counter() - t0
                 print(json.dumps(line), flush=True)
