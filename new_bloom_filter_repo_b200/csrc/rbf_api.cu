@@ -39,15 +39,15 @@ struct rbf_ctx {
     cudaStream_t st_k1 = nullptr;     // pipelined encode: K1 of the later ranges + the witness memset run here, beside K2 on `st`
     cudaStream_t st_d2h = nullptr;    // rbf_stream_encode_host: result copies of chunk i overlap the kernels of chunk i+1
     cudaEvent_t ev_fork = nullptr, ev_wit = nullptr, ev_k1[8] = {nullptr}, ev_d2h = nullptr;
-    int encode_ranges = 1;            // rbf_stream_encode: K1/K2 pipelined over this many ranges of pairs (1 = serial, the default: K1 (HBM)
-                                      // and K2 (L2 atomics) compete when they overlap)
+    int encode_ranges = 1;            // rbf_stream_encode: K1/K2 pipelined over this many ranges of pairs (1 = serial, the default; a K2 CTA
+                                      // takes a whole SM's shared memory, so K1 and K2 overlap on different SMs)
     int k1_ctas_per_sm = 32;          // grid cap of K1 (pipelined encodes use pipe_k1_ctas_per_sm so that K2 finds room beside it)
     int pipe_k1_ctas_per_sm = 4;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaDeviceProp prop;
     int sm_count = 0;
     int k1_variant = 0;
-    int insert_variant = 1; // 1: dense warp-compacted K2 (one RED.OR per probe; default); 0: per-lane K2
+    int insert_variant = 1; // 1: dense warp-compacted K2 building the arrays in shared memory (default); 0: per-lane K2, RED.OR into L2
     int query_variant = 5;  // 0: per-lane; 1: staged A->B->C rings, L2 tail; 2, 3, 4: as 5; 5: decade tiles with carried stage-B
                             // batches (half tiles for 2^23 < m <= 2^24, ring kernel beyond); 6: half-decade tiles for every m <= 2^24
     int k1_only = 0;        // stop after K1 (mask + counts): VideoFrameCompressor._calculate_frame_diff
@@ -55,6 +55,8 @@ struct rbf_ctx {
     int query_smem_cap = 0;
     int query_warps = 0;    // warps per CTA of the tile query kernel (0 = its compiled maximum, 28)
     int kq_ranges = 1;      // > 1: K2 of range r+1 runs beside K3 of range r (see stream_encode_pipelined)
+    int k2_clusters[9] = {0};   // resident K2 clusters of 1..8 CTAs, measured by the first K2 launch of each shape.  Not at
+                                // creation: querying it there slowed 8K K3 (which never uses this kernel) by 12 %, cause unknown
     char err[512];
     int64_t launches = 0, h2d = 0, d2h = 0;
     std::vector<void*> scratch;
@@ -502,7 +504,7 @@ extern "C" int rbf_compress_mask(rbf_ctx* c, const uint8_t* mask, uint64_t n, co
     CK(c, cudaMemcpyAsync(d_prefix, h_prefix, 8, cudaMemcpyHostToDevice, c->st));
     CK(c, cudaMemsetAsync(d_bits, 0, bit_words_padded(l) * 4, c->st));
     CK(c, cudaMemsetAsync(d_wit, 0, mw * 4, c->st));
-    LAUNCH(c, launch_insert(d_job, 1, ncent, c->insert_variant, c->sm_count, c->st));
+    LAUNCH(c, launch_insert(d_job, 1, ncent, (uint32_t)l, c->insert_variant, c->sm_count, c->k2_clusters, c->st));
     LAUNCH(c, launch_query(d_job, d_prefix, 1, ncent, (uint32_t)l, c->query_variant, c->sm_count, c->query_smem_cap, c->query_warps, c->st));
     LAUNCH(c, launch_witness(d_job, 1, ncent, c->sm_count, (uint32_t*)((uint8_t*)d_small + 1024), d_cnt + 1, c->st)); c->launches += 2;
     CK(c, cudaMemcpyAsync(h_cnt, d_cnt, 16, cudaMemcpyDeviceToHost, c->st)); c->d2h += 16;
@@ -830,7 +832,7 @@ static int stream_encode_range(rbf_stream* s, uint32_t first, uint32_t count, ui
     if (int r = wait_pack(c)) return r;                  // the slots of the last all-gather are packed
     if (int r = stream_clear_outputs(s, first, count, rt.max_l, c->st)) return r;
     if (record_events) CK(c, cudaEventRecord(s->ev[2], c->st));
-    LAUNCH(c, launch_insert(s->d_jobs + first, (int)count, ncent, c->insert_variant, c->sm_count, c->st));
+    LAUNCH(c, launch_insert(s->d_jobs + first, (int)count, ncent, rt.max_l, c->insert_variant, c->sm_count, c->k2_clusters, c->st));
     if (record_events) CK(c, cudaEventRecord(s->ev[3], c->st));
     LAUNCH(c, launch_query(s->d_jobs + first, s->d_prefix + pfx, (int)count, rt.total_cent, rt.max_l, c->query_variant, c->sm_count,
                            c->query_smem_cap, c->query_warps, c->st));
@@ -855,8 +857,9 @@ static int ensure_pipe_streams(rbf_ctx* c) {
 
 // The resident-stream encode, pipelined: K1 has no host dependency, so K1 of ALL ranges is enqueued up front on a second
 // stream; as soon as a range's counts have landed the host derives its (k, l, T) and enqueues that range's K2 on the main
-// stream, where it runs BESIDE K1 of the later ranges (K1 is HBM-bound with a grid that leaves SM slots free, K2 is
-// issue/atomics-bound), and the host round trip is hidden behind both.  K3 and K3b are single launches over all pairs.
+// stream, where it can run beside K1 of the later ranges (K1 is HBM-bound with a grid that leaves SM slots free; K2's CTAs
+// take a whole SM's shared memory, so they start on SMs K1 leaves free), and the host round trip is hidden behind both.
+// K3 and K3b are single launches over all pairs.
 static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t* prev_idx, const uint32_t* curr_idx,
                                    double threshold, const rbf_seeds* sd, const double* kov, const uint64_t* lov) {
     rbf_ctx* c = s->c;
@@ -894,9 +897,9 @@ static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t
     RangeTotals all;
     uint32_t base_cent = 0;
     bool first_k2 = true;
-    // K2 || K3 mode (kq_ranges > 1, serial K1): K2 is bound by L2 atomics with the SMs mostly waiting, K3 by instruction issue with
-    // L2 idle; K2 of range q+1 is enqueued on the second stream and runs BESIDE K3 of range q (K3 is then launched with fewer
-    // warps and a little less shared memory -- options query_warps / query_smem_bytes -- so that one K2 CTA fits next to it).
+    // K2 || K3 mode (kq_ranges > 1, serial K1): K2 of range q+1 is enqueued on the second stream beside K3 of range q.  Both
+    // kernels take nearly all of an SM's shared memory, so a K2 CTA only starts on an SM without a K3 CTA: the two stages
+    // share the GPU by SMs, not within one.
     uint32_t Q = (R == 1u && !s->k1_only) ? (uint32_t)c->kq_ranges : 1u;
     if (Q > 8u) Q = 8u;
     if (pairs < 8u * Q) Q = 1u;
@@ -915,7 +918,7 @@ static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t
         if (first_k2) { if (int e = wait_pack(c)) return e; }
         if (int e = stream_clear_outputs(s, f, cnt, rt.max_l, c->st)) return e;
         if (first_k2) { CK(c, cudaEventRecord(s->ev[2], c->st)); first_k2 = false; }
-        if (!kq) LAUNCH(c, launch_insert(s->d_jobs + f, (int)cnt, ncent, c->insert_variant, c->sm_count, c->st));
+        if (!kq) LAUNCH(c, launch_insert(s->d_jobs + f, (int)cnt, ncent, rt.max_l, c->insert_variant, c->sm_count, c->k2_clusters, c->st));
     }
     all.total_cent = base_cent;
     s->last_max_l = all.max_l;
@@ -941,7 +944,7 @@ static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t
         CK(c, cudaStreamWaitEvent(c->st_k1, c->ev_fork, 0));
         for (uint32_t q = 0; q < Q; q++) {
             const uint32_t f = qlo[q], cnt = qlo[q + 1] - qlo[q];
-            LAUNCH(c, launch_insert(s->d_jobs + f, (int)cnt, ncent, c->insert_variant, c->sm_count, c->st_k1));
+            LAUNCH(c, launch_insert(s->d_jobs + f, (int)cnt, ncent, all.max_l, c->insert_variant, c->sm_count, c->k2_clusters, c->st_k1));
             CK(c, cudaEventRecord(c->ev_k1[q], c->st_k1));
             CK(c, cudaStreamWaitEvent(c->st, c->ev_k1[q], 0));
             if (q == 0) CK(c, cudaEventRecord(s->ev[3], c->st));

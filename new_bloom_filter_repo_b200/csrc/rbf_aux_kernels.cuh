@@ -175,7 +175,7 @@ __global__ void k_items_u32(const FrameJob* __restrict__ job, const uint32_t* __
         const uint64_t h1 = finish(cen.kind, decade_state(cen, century_state(cen, K.s1), K.s1, x), K.s1, y);
         const uint64_t h2 = finish(cen.kind, decade_state(cen, century_state(cen, K.s2), K.s2, x), K.s2, y);
         const uint64_t hA = K.has_act ? finish(cen.kind, decade_state(cen, century_state(cen, K.sA), K.sA, x), K.sA, y) : 0ull;
-        if (insert) insert_hashes(J.bits, K, h1, h2, hA);
+        if (insert) insert_hashes(GlobalBits{J.bits}, K, h1, h2, hA);
         else result[t] = (uint8_t)check_hashes_global(J.bits, K, h1, h2, hA);
     }
 }
@@ -199,7 +199,7 @@ __global__ void k_items_str(const FrameJob* __restrict__ job, const uint8_t* __r
         } else {
             const uint64_t h1 = xxh64_bytes(s, len, K.s1), h2 = xxh64_bytes(s, len, K.s2);
             const uint64_t hA = K.has_act ? xxh64_bytes(s, len, K.sA) : 0ull;
-            if (insert) insert_hashes(J.bits, K, h1, h2, hA);
+            if (insert) insert_hashes(GlobalBits{J.bits}, K, h1, h2, hA);
             else result[t] = (uint8_t)check_hashes_global(J.bits, K, h1, h2, hA);
         }
     }

@@ -201,17 +201,58 @@ cudaError_t launch_threshold(const PairJob* d_pairs, int F, uint32_t npix, int c
     return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_insert(const FrameJob* d_jobs, int F, uint32_t max_centuries, int variant, int sm_count, cudaStream_t st) {
+static cudaLaunchConfig_t insert_cluster_config(uint32_t cs, uint32_t units, cudaStream_t st, cudaLaunchAttribute* attr) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(cs, units);
+    cfg.blockDim = dim3(K2_THREADS);
+    cfg.dynamicSmemBytes = K2_SMEM_BYTES;
+    cfg.stream = st;
+    attr->id = cudaLaunchAttributeClusterDimension;
+    attr->val.clusterDim.x = cs; attr->val.clusterDim.y = 1; attr->val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cfg;
+}
+
+// resident clusters of cs CTAs; 0 means the shape cannot be scheduled
+static cudaError_t insert_cluster_occupancy(uint32_t cs, int* clusters) {
+    cudaError_t e = cudaFuncSetAttribute(k_insert_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)K2_SMEM_BYTES);
+    if (e != cudaSuccess) return e;
+    cudaLaunchAttribute attr;
+    const cudaLaunchConfig_t cfg = insert_cluster_config(cs, 1u, nullptr, &attr);
+    return cudaOccupancyMaxActiveClusters(clusters, k_insert_cluster, &cfg);
+}
+
+cudaError_t launch_insert(const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t max_l_bits, int variant, int sm_count,
+                          int* k2_clusters, cudaStream_t st) {
     if (F <= 0 || max_centuries == 0) return cudaSuccess;
-    if (variant >= 1) {                                   // dense, warp-compacted insert
-        // One CTA per 4 slabs, no grid cap: CTAs are dispatched frame after frame, so the bit arrays being written at any time
-        // stay in L2.  A capped grid-stride form spreads over all F frames at once, and 299 4K arrays (72 MB) overflow the
-        // H100's 50 MB L2 (K2 8.3 -> 5.0 ms per 299 pairs).
+    const uint32_t words = (uint32_t)(((uint64_t)max_l_bits + 31u) >> 5);
+    if (variant >= 1 && words > 2u * K2_MAX_CS * K2_WORDS) {   // less than half of the array would be on chip: RED.OR into L2
         const uint32_t nslab = (max_centuries + 31u) / 32u;
-        const uint32_t bx = (nslab + I2_WARPS - 1) / I2_WARPS;
-        dim3 grid(bx, (unsigned)F);
+        dim3 grid((nslab + I2_WARPS - 1) / I2_WARPS, (unsigned)F);
         k_insert2<<<grid, I2_WARPS * 32, 0, st>>>(d_jobs);
         return cudaGetLastError();
+    }
+    if (variant >= 1) {                                   // dense, warp-compacted insert into (cluster) shared memory
+        uint32_t cs = (words + K2_WORDS - 1u) / K2_WORDS;
+        if (cs < 1u) cs = 1u;
+        if (cs > (uint32_t)K2_MAX_CS) cs = K2_MAX_CS;    // the rest of the array is set with RED.OR in L2
+        // Full waves of resident clusters take one frame each; the frames of the last, partial wave (all of them when F is small)
+        // get R copies each so that they still fill the GPU, with at least K2_WARPS slabs per CTA.
+        if (k2_clusters[cs] == 0) {                       // first launch of this shape: measure it once, and refuse it if it does not fit
+            cudaError_t e = insert_cluster_occupancy(cs, &k2_clusters[cs]);
+            if (e != cudaSuccess) return e;
+            if (k2_clusters[cs] < 1) { k2_clusters[cs] = 0; return cudaErrorInvalidConfiguration; }
+        }
+        const uint32_t slots = (uint32_t)k2_clusters[cs], full = (uint32_t)F / slots * slots, rem = (uint32_t)F - full;
+        const uint32_t nslab = (max_centuries + 31u) / 32u;
+        const uint32_t useful = (nslab + cs * K2_WARPS - 1u) / (cs * K2_WARPS);
+        uint32_t copies = rem ? slots / rem : 1u;
+        if (copies > useful) copies = useful;
+        if (copies < 1u) copies = 1u;
+        cudaLaunchAttribute attr;
+        const cudaLaunchConfig_t cfg = insert_cluster_config(cs, full + rem * copies, st, &attr);
+        return cudaLaunchKernelEx(&cfg, k_insert_cluster, d_jobs, full, copies);
     }
     uint32_t bx = (max_centuries + 255u) / 256u;
     const uint32_t cap = (uint32_t)(sm_count * 16);

@@ -71,7 +71,10 @@ struct DeflateCopy {
 cudaError_t launch_threshold(const PairJob* d_pairs, int F, uint32_t npix, int channels, int sample_bytes,
                              int thr_int, int any_mode, int gray_mode, uint32_t* d_ones, uint32_t* d_resid, int variant,
                              bool chain, int sm_count, int ctas_per_sm, cudaStream_t st);
-cudaError_t launch_insert(const FrameJob* d_jobs, int F, uint32_t max_centuries, int variant, int sm_count, cudaStream_t st);
+// K2: variant 1 builds the arrays in (cluster) shared memory.  k2_clusters[1..8]: resident clusters of that many CTAs, 0 until
+// the first launch of the shape measures it with cudaOccupancyMaxActiveClusters (a shape that cannot be scheduled is an error)
+cudaError_t launch_insert(const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t max_l_bits, int variant, int sm_count,
+                          int* k2_clusters, cudaStream_t st);
 cudaError_t launch_query(const FrameJob* d_jobs, const uint32_t* d_cent_prefix, int F, uint32_t total_centuries,
                          uint32_t max_l_bits, int variant, int sm_count, int smem_bytes_cap, int tile_warps, cudaStream_t st);
 cudaError_t launch_witness(const FrameJob* d_jobs, int F, uint32_t max_centuries, int sm_count, uint32_t* d_scratch, uint32_t* d_wlen,
