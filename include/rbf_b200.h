@@ -189,6 +189,30 @@ int rbf_stream_gather_changed(rbf_stream* s, uint32_t pairs, uint8_t* values_out
 int rbf_stream_apply_diff(rbf_stream* s, uint32_t base_frame, uint32_t out_frame, const uint8_t* mask_packed_little,
                           const uint8_t* values, uint64_t values_bytes, uint64_t* applied_pixels);
 int rbf_stream_download(rbf_stream* s, uint32_t frame, void* host_out);
+/* ---- K4b / K4c: a group of inter frames decoded at once (ImprovedVideoCompressor.decompress_video)
+ * rbf_stream_decode_masks  BloomFilterCompressor.decompress (ivc:268-307) of `count` pairs in one query + expand launch: pair i's
+ *     payload bytes as stored, in slots like those of rbf_stream_fetch_batch -- bitmaps_packbits + i*bitmap_slot_bytes holds
+ *     np.packbits of its l[i]-bit array, or, when raw[i], np.packbits of the n-bit mask itself (ivc:215-225); the witness
+ *     likewise (wlen[i] bits, empty for raw pairs; witness_packbits may be NULL when witness_slot_bytes is 0).  One H2D copy
+ *     per kind; k[i] is the payload's float64 k*.  Slots are at most the stream's mask slot (see rbf_stream_fetch_batch).  The
+ *     masks land in the stream's mask slots 0..count-1.  consumed_out[i] = positions that passed the Bloom test (as
+ *     rbf_decompress_mask reports it; 0 for raw pairs), ones_out[i] = set bits of the decoded mask.  One synchronisation.
+ *     The bit-array, witness and mask slots no longer hold an encode's outputs afterwards: fetch / gather / decode_verify
+ *     refuse until the next rbf_stream_encode.
+ * rbf_stream_apply_chain   VideoFrameCompressor._apply_frame_diff (ivc:849-909) along a chain: frame base_frame+1+i = frame
+ *     base_frame+i with mask slot i applied (its set pixels replaced, in rank order, by the value bytes
+ *     values[value_offsets[i], value_offsets[i+1])), i < count; one H2D copy of the values, one synchronisation.  Frame slots
+ *     are taken modulo max_frames, so a chain may continue from the last frame of the previous one wherever it sits; count <
+ *     max_frames.  ivc:882 per pair: pair i is applied only if its mask's popcount x pixel bytes equals its value bytes; the
+ *     first pair that fails gets applied_out[i] = 0 and no frame from there on is written.  applied_out[i] = pixels applied.
+ * rbf_stream_download_batch  frames first .. first+count-1 (slots modulo max_frames) into one contiguous host array, one
+ *     synchronisation. */
+int rbf_stream_decode_masks(rbf_stream* s, uint32_t count, const uint8_t* bitmaps_packbits, uint64_t bitmap_slot_bytes,
+                            const uint8_t* witness_packbits, uint64_t witness_slot_bytes, const uint64_t* l, const uint64_t* wlen,
+                            const double* k, const uint8_t* raw, const rbf_seeds* seeds, uint64_t* consumed_out, uint64_t* ones_out);
+int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values, const uint64_t* value_offsets,
+                           uint64_t* applied_out);
+int rbf_stream_download_batch(rbf_stream* s, uint32_t first, uint32_t count, void* host_out);
 /* N3  the 5x5 median of cv2.medianBlur in VideoFrameCompressor._estimate_noise_level (ivc:738): replicated border, 13th
  *     smallest of 25, exact for uint8 / uint16.  The float32 std of (frame - median) stays in numpy (ivc:741-744). */
 int rbf_median_blur5(rbf_ctx* ctx, const void* plane_in, uint32_t height, uint32_t width, uint32_t sample_bytes, void* plane_out);

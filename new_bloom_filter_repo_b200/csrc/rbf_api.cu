@@ -1233,6 +1233,146 @@ extern "C" int rbf_stream_download(rbf_stream* s, uint32_t frame, void* host_out
     return RBF_OK;
 }
 
+// ------------------------------------------------------------------------------------------
+// K4b / K4c batched: the inter frames of a group decoded with one query + expand and rebuilt along the chain in one sweep
+// ------------------------------------------------------------------------------------------
+extern "C" int rbf_stream_decode_masks(rbf_stream* s, uint32_t count, const uint8_t* bitmaps, uint64_t bitmap_slot,
+                                       const uint8_t* witness, uint64_t witness_slot, const uint64_t* l, const uint64_t* wlen,
+                                       const double* k, const uint8_t* raw, const rbf_seeds* sd, uint64_t* consumed_out,
+                                       uint64_t* ones_out) {
+    if (!s || !bitmaps || !l || !wlen || !k || !raw || !sd || !consumed_out || !ones_out || (witness_slot && !witness))
+        return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_decode_masks: NULL");
+    rbf_ctx* c = s->c;
+    const uint64_t n = s->npix, stride = s->mask_stride_w * 4;
+    if (count == 0 || count > s->max_pairs) return set_err(c, RBF_ERR_INVALID, "%u pairs for a stream of %u", count, s->max_pairs);
+    if (bitmap_slot == 0 || bitmap_slot > stride || witness_slot > stride)
+        return set_err(c, RBF_ERR_INVALID, "slots of %llu / %llu bytes exceed the device slot of %llu", (unsigned long long)bitmap_slot,
+                       (unsigned long long)witness_slot, (unsigned long long)stride);
+    for (uint32_t i = 0; i < count; i++) {
+        if (raw[i]) {
+            if (bitmap_slot < (n + 7) / 8) return set_err(c, RBF_ERR_INVALID, "pair %u: a raw mask needs %llu bytes", i, (unsigned long long)((n + 7) / 8));
+        } else if (l[i] == 0 || l[i] > 0xffffffffULL || l[i] > 8 * bitmap_slot || wlen[i] == 0 || wlen[i] > 8 * witness_slot || !(k[i] >= 0.0)) {
+            return set_err(c, RBF_ERR_INVALID, "pair %u: bad l / wlen / k", i);
+        }
+    }
+    CK(c, cudaSetDevice(c->device));
+    if (int r = wait_pack(c)) return r;                  // the bit arrays are overwritten
+    void* d_cnt;
+    if (int r = scratch_get(c, 21, 8 * (size_t)count, &d_cnt)) return r;
+    uint32_t* d_consumed = (uint32_t*)d_cnt;
+    uint32_t* d_ones = d_consumed + count;
+    CK(c, cudaMemcpy2DAsync(s->d_bits, stride, bitmaps, bitmap_slot, bitmap_slot, count, cudaMemcpyHostToDevice, c->st));
+    c->h2d += (int64_t)(bitmap_slot * count);
+    if (witness_slot) {
+        CK(c, cudaMemcpy2DAsync(s->d_wit, stride, witness, witness_slot, witness_slot, count, cudaMemcpyHostToDevice, c->st));
+        c->h2d += (int64_t)(witness_slot * count);
+    }
+    // packbits order -> LSB-first words.  k_bitrev reverses each byte in place, so whatever lies past a slot is only reordered,
+    // and nothing reads a bit array at or past bit l or a witness at or past bit wlen
+    LAUNCH(c, launch_bitrev(s->d_bits, s->mask_stride_w * count, c->sm_count, c->st));
+    if (witness_slot) LAUNCH(c, launch_bitrev(s->d_wit, s->mask_stride_w * count, c->sm_count, c->st));
+    CK(c, cudaMemsetAsync(s->d_mask, 0, stride * count, c->st));       // K4b ORs into the mask slots
+    CK(c, cudaMemsetAsync(d_cnt, 0, 8 * (size_t)count, c->st));
+    const uint32_t ncent = (uint32_t)((n + 99) / 100);
+    uint32_t total_cent = 0, max_l = 0, coded = 0;
+    s->h_prefix[0] = 0;
+    for (uint32_t i = 0; i < count; i++) {
+        FrameJob& J = s->h_jobs[i];
+        memset(&J, 0, sizeof J);
+        J.n = (uint32_t)n;
+        J.bits = s->d_bits + (size_t)i * s->mask_stride_w;
+        J.witness = s->d_wit + (size_t)i * s->mask_stride_w;
+        J.pass = s->d_pass + (size_t)i * s->pass_stride_w;
+        J.out_mask = s->d_mask + (size_t)i * s->mask_stride_w;
+        if (!raw[i]) {                                    // the payload's float64 k (ivc:275-279)
+            job_set_filter(J, l[i], k[i], *sd);
+            J.wlen_in = (uint32_t)wlen[i];
+            total_cent += ncent; coded++;
+            if (l[i] > max_l) max_l = (uint32_t)l[i];
+        }
+        s->h_prefix[i + 1] = total_cent;
+    }
+    CK(c, cudaMemcpyAsync(s->d_jobs, s->h_jobs, sizeof(FrameJob) * count, cudaMemcpyHostToDevice, c->st));
+    if (coded) {
+        CK(c, cudaMemcpyAsync(s->d_prefix, s->h_prefix, 4 * ((size_t)count + 1), cudaMemcpyHostToDevice, c->st));
+        LAUNCH(c, launch_query(s->d_jobs, s->d_prefix, (int)count, total_cent, max_l, c->query_variant, c->sm_count, c->query_smem_cap,
+                               c->query_warps, c->st));
+        LAUNCH(c, launch_expand(s->d_jobs, (int)count, ncent, c->sm_count, s->d_chunkcnt, d_consumed, c->st));
+        c->launches += 1;
+    }
+    if (coded < count) LAUNCH(c, launch_raw_masks(s->d_jobs, (int)count, (uint32_t)n, c->st));
+    LAUNCH(c, launch_mask_popcount(s->d_mask, s->mask_stride_w, (uint32_t)n, (int)count, d_ones, c->sm_count, c->st));
+    std::vector<uint32_t> h(2 * (size_t)count);
+    CK(c, cudaMemcpyAsync(h.data(), d_cnt, 8 * (size_t)count, cudaMemcpyDeviceToHost, c->st));
+    c->d2h += 8 * (int64_t)count;
+    CK(c, cudaStreamSynchronize(c->st));
+    for (uint32_t i = 0; i < count; i++) { consumed_out[i] = raw[i] ? 0 : h[i]; ones_out[i] = h[count + i]; }
+    // the slots no longer hold the outputs of an encode: refuse fetch / gather / decode_verify until the next one, and let the next
+    // encode clear what was written here
+    s->last_pairs = 0; s->last_max_l = 0; s->staged = false;
+    const size_t bh = align_up((size_t)bitmap_slot + 64, 128), wh = align_up((size_t)witness_slot + 64, 128);
+    if (bh > s->bits_hwm) s->bits_hwm = bh;
+    if (witness_slot && wh > s->wit_hwm) s->wit_hwm = wh;
+    return RBF_OK;
+}
+
+extern "C" int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
+                                      const uint64_t* value_offsets, uint64_t* applied_out) {
+    if (!s || !value_offsets || !applied_out) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_apply_chain: NULL");
+    rbf_ctx* c = s->c;
+    if (count == 0 || count > s->max_pairs || count >= s->max_frames || base_frame >= s->max_frames)
+        return set_err(c, RBF_ERR_INVALID, "chain of %u frames from slot %u does not fit a store of %u frames / %u pairs", count,
+                       base_frame, s->max_frames, s->max_pairs);
+    for (uint32_t i = 0; i < count; i++)
+        if (value_offsets[i + 1] < value_offsets[i]) return set_err(c, RBF_ERR_INVALID, "value offsets decrease at pair %u", i);
+    const uint64_t vbytes = value_offsets[count];
+    if (vbytes && !values) return set_err(c, RBF_ERR_INVALID, "rbf_stream_apply_chain: values is NULL");
+    CK(c, cudaSetDevice(c->device));
+    const uint32_t ntiles = (uint32_t)((s->npix + AP_TILE_PX - 1) / AP_TILE_PX);
+    void *d_vals, *d_small, *d_pfx;
+    int rc;
+    const size_t small = align_up(8 * ((size_t)count + 1), 16) + 4 * ((size_t)count + 1);
+    if ((rc = scratch_get(c, 8, (size_t)vbytes + 256, &d_vals)) || (rc = scratch_get(c, 22, small, &d_small)) ||
+        (rc = scratch_get(c, 23, 4 * (size_t)count * ntiles, &d_pfx)))
+        return rc;
+    uint64_t* d_off = (uint64_t*)d_small;
+    uint32_t* d_res = (uint32_t*)((uint8_t*)d_small + align_up(8 * ((size_t)count + 1), 16));   // [0] first_bad, [1 + i] totals
+    if (vbytes) { CK(c, cudaMemcpyAsync(d_vals, values, (size_t)vbytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)vbytes; }
+    CK(c, cudaMemcpyAsync(d_off, value_offsets, 8 * ((size_t)count + 1), cudaMemcpyHostToDevice, c->st));
+    c->h2d += 8 * ((int64_t)count + 1);
+    CK(c, cudaMemsetAsync(d_res, 0xff, 4, c->st));
+    ApplyChain A;
+    A.masks = s->d_mask; A.mask_stride_w = s->mask_stride_w;
+    A.frames = s->d_frames; A.frame_stride = s->frame_stride;
+    A.max_frames = s->max_frames; A.base = base_frame;
+    A.npix = (uint32_t)s->npix; A.ntiles = ntiles; A.count = count; A.pix_bytes = s->C * s->S;
+    A.values = (const uint8_t*)d_vals; A.value_off = d_off;
+    A.tile_pfx = (uint32_t*)d_pfx; A.totals = d_res + 1; A.first_bad = d_res;
+    LAUNCH(c, launch_apply_chain(A, c->sm_count, c->st));
+    c->launches += 2;                                   // tile count + tile scan
+    std::vector<uint32_t> h((size_t)count + 1);
+    CK(c, cudaMemcpyAsync(h.data(), d_res, 4 * ((size_t)count + 1), cudaMemcpyDeviceToHost, c->st));
+    c->d2h += 4 * ((int64_t)count + 1);
+    CK(c, cudaStreamSynchronize(c->st));
+    for (uint32_t i = 0; i < count; i++) applied_out[i] = i < h[0] ? h[1 + i] : 0;
+    return RBF_OK;
+}
+
+extern "C" int rbf_stream_download_batch(rbf_stream* s, uint32_t first, uint32_t count, void* host_out) {
+    if (!s || !host_out || first >= s->max_frames || count == 0 || count > s->max_frames)
+        return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_download_batch: bad argument");
+    rbf_ctx* c = s->c;
+    const uint32_t head = count < s->max_frames - first ? count : s->max_frames - first;   // slots wrap as in rbf_stream_apply_chain
+    CK(c, cudaMemcpy2DAsync(host_out, s->frame_bytes, s->d_frames + (size_t)first * s->frame_stride, s->frame_stride, s->frame_bytes,
+                            head, cudaMemcpyDeviceToHost, c->st));
+    if (head < count)
+        CK(c, cudaMemcpy2DAsync((uint8_t*)host_out + (size_t)head * s->frame_bytes, s->frame_bytes, s->d_frames, s->frame_stride,
+                                s->frame_bytes, count - head, cudaMemcpyDeviceToHost, c->st));
+    c->d2h += (int64_t)s->frame_bytes * count;
+    CK(c, cudaStreamSynchronize(c->st));
+    return RBF_OK;
+}
+
 
 // ------------------------------------------------------------------------------------------
 // N3: cv2.medianBlur(frame, 5) of VideoFrameCompressor._estimate_noise_level (ivc:738)

@@ -6,6 +6,7 @@
 //   K3  k_query          Bloom test of ALL n positions -> pass mask                 (ivc:245-253, ivc:116-138)
 //   K3b k_witness        ordered witness = mask bits at passing positions           (ivc:253)
 //   K4b k_expand         decode: out[i] = witness[rank(i)] for passing i            (ivc:299-304)
+//   K4c k_apply_sweep    a group's decoded masks applied along the frame chain      (ivc:849-909)
 //   N4  k_deflate_segments / k_deflate_concat   zlib streams of host or device buffers (rbf_deflate.cuh)
 //
 // The Bloom bit array of the frame being queried is staged into shared memory with
@@ -13,7 +14,7 @@
 // CTA is probed through L2.  Integer hashing / bit tests only: no tensor cores.
 //
 // One translation unit: this file holds the PTX helpers and the launchers; the kernels live in
-// rbf_k1_threshold.cuh, rbf_k2_insert.cuh, rbf_k3_query.cuh, rbf_k3b_witness.cuh, rbf_aux_kernels.cuh and rbf_deflate.cuh.
+// rbf_k1_threshold.cuh, rbf_k2_insert.cuh, rbf_k3_query.cuh, rbf_k3b_witness.cuh, rbf_aux_kernels.cuh, rbf_deflate.cuh and rbf_k4c_apply.cuh.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -108,6 +109,7 @@ __device__ __forceinline__ void or_bits128(uint32_t* __restrict__ W, uint64_t bi
 #include "rbf_k3b_witness.cuh"
 #include "rbf_aux_kernels.cuh"
 #include "rbf_deflate.cuh"
+#include "rbf_k4c_apply.cuh"
 
 // ------------------------------------------------------------------------------------------
 // launchers
@@ -391,6 +393,45 @@ cudaError_t launch_gather_scatter(const GatherJob* d_jobs, int F, int scatter, u
     default: return cudaErrorInvalidValue;
     }
     return cudaGetLastError();
+}
+cudaError_t launch_raw_masks(const FrameJob* d_jobs, int F, uint32_t npix, cudaStream_t st) {
+    if (F <= 0 || npix == 0) return cudaSuccess;
+    unsigned gx = (((npix + 31u) >> 5) + 255u) / 256u;
+    if (gx > 64u) gx = 64u;
+    k_raw_masks<<<dim3(gx, (unsigned)F), 256, 0, st>>>(d_jobs);
+    return cudaGetLastError();
+}
+cudaError_t launch_mask_popcount(const uint32_t* d_masks, size_t stride_w, uint32_t npix, int F, uint32_t* d_out, int sm_count,
+                                 cudaStream_t st) {
+    if (F <= 0 || npix == 0) return cudaSuccess;
+    const uint32_t nwords = (npix + 31u) >> 5;
+    unsigned gx = grid_for(nwords, 256, sm_count);
+    if (gx > 64u) gx = 64u;
+    k_mask_popcount<<<dim3(gx, (unsigned)F), 256, 0, st>>>(d_masks, stride_w, nwords, d_out);
+    return cudaGetLastError();
+}
+template <int PB>
+static cudaError_t launch_apply_sweep_t(const ApplyChain& A, int sm_count, cudaStream_t st) {
+    int per_sm = 1;
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_apply_sweep<PB>, AP_THREADS, 0);
+    if (e != cudaSuccess) return e;
+    if (per_sm < 1) per_sm = 1;
+    const uint32_t slots = (uint32_t)(sm_count > 0 ? sm_count : 1) * (uint32_t)per_sm;
+    const uint32_t rounds = (A.ntiles + slots - 1u) / slots;          // every CTA sweeps the same number of tiles, or one fewer
+    k_apply_sweep<PB><<<(A.ntiles + rounds - 1u) / rounds, AP_THREADS, 0, st>>>(A);
+    return cudaGetLastError();
+}
+cudaError_t launch_apply_chain(const ApplyChain& A, int sm_count, cudaStream_t st) {
+    if (A.count == 0 || A.ntiles == 0) return cudaSuccess;
+    k_tile_count<<<dim3((A.ntiles + 7u) / 8u, A.count), 256, 0, st>>>(A);
+    k_tile_scan<<<A.count, 1024, 0, st>>>(A);
+    switch (A.pix_bytes) {
+    case 1: return launch_apply_sweep_t<1>(A, sm_count, st);
+    case 2: return launch_apply_sweep_t<2>(A, sm_count, st);
+    case 3: return launch_apply_sweep_t<3>(A, sm_count, st);
+    case 6: return launch_apply_sweep_t<6>(A, sm_count, st);
+    default: return cudaErrorInvalidValue;
+    }
 }
 cudaError_t launch_median5(const void* d_in, uint32_t pix_stride, uint32_t H, uint32_t W, int sample_bytes, void* d_out, cudaStream_t st) {
     if (H == 0 || W == 0) return cudaSuccess;

@@ -46,6 +46,25 @@ struct GatherJob {
 };
 
 
+// K4c (rbf_k4c_apply.cuh): a chain of decoded masks applied to one base frame, frames base+1 .. base+count
+static constexpr int AP_THREADS = 128;
+static constexpr uint32_t AP_TILE_WORDS = AP_THREADS;
+static constexpr uint32_t AP_TILE_PX = 32u * AP_TILE_WORDS;     // 4096 px: 4 / 8 / 12 / 24 KB of shared memory at 1 / 2 / 3 / 6 B per pixel
+
+struct ApplyChain {
+    const uint32_t* masks;      // mask of pair t at masks + t * mask_stride_w
+    size_t mask_stride_w;
+    uint8_t* frames;            // the stream's frame store
+    size_t frame_stride;
+    uint32_t max_frames, base;  // slots; pair t reads slot (base + t) % max_frames and writes (base + t + 1) % max_frames
+    uint32_t npix, ntiles, count, pix_bytes;
+    const uint8_t* values;      // rank-ordered pixel values of every pair, back to back
+    const uint64_t* value_off;  // [count + 1] byte offsets of each pair's values
+    uint32_t* tile_pfx;         // [count][ntiles]: set bits per tile (k_tile_count), then set bits of the earlier tiles (k_tile_scan)
+    uint32_t* totals;           // [count] set bits per pair
+    uint32_t* first_bad;        // first pair whose value bytes do not match its mask (UINT32_MAX: none); pairs from there are not applied
+};
+
 // N4 deflate (rbf_deflate.cuh): one segment of at most 64 KiB per CTA, and the join of coded segments into zlib streams
 static constexpr uint32_t kDeflateSeg = 65536;         // segment size (bytes); the layout is pinned in rbf_deflate.cuh
 // worst-case output of one segment of n bytes (0 < n <= kDeflateSeg): stored blocks plus the sync flush
@@ -84,6 +103,12 @@ cudaError_t launch_expand(const FrameJob* d_jobs, int F, uint32_t max_centuries,
 uint32_t gather_chunks(uint32_t npix);
 cudaError_t launch_gather_scatter(const GatherJob* d_jobs, int F, int scatter, uint32_t npix, uint32_t pix_bytes, uint32_t* d_counts,
                                   uint32_t* d_totals, cudaStream_t st);
+// decode side of a group (rbf_k4c_apply.cuh): masks of the raw-passthrough jobs (l == 0) from their bitmap slots; set bits per mask
+cudaError_t launch_raw_masks(const FrameJob* d_jobs, int F, uint32_t npix, cudaStream_t st);
+cudaError_t launch_mask_popcount(const uint32_t* d_masks, size_t stride_w, uint32_t npix, int F, uint32_t* d_out, int sm_count,
+                                 cudaStream_t st);
+// K4c: tile counts, tile scan (+ the ivc:882 check) and the chained sweep; *A.first_bad must hold UINT32_MAX before the launch
+cudaError_t launch_apply_chain(const ApplyChain& A, int sm_count, cudaStream_t st);
 cudaError_t launch_median5(const void* d_in, uint32_t pix_stride, uint32_t H, uint32_t W, int sample_bytes, void* d_out, cudaStream_t st);
 cudaError_t launch_bitrev(uint32_t* d_words, size_t nwords, int sm_count, cudaStream_t st);
 cudaError_t launch_unpack_bits(const uint32_t* d_words, uint8_t* d_out, size_t nbits, int sm_count, cudaStream_t st);

@@ -347,6 +347,20 @@ _INTER_TAG = b"\xff\xff\xff\xffRBF2"      # current: raw-passthrough masks zlib-
 # the reference's decoder knows keyframes only (ivc:1124); files written with keyframe_interval=1 are interchangeable.
 
 
+class _InterPayload:
+    """The fields of one inter-frame payload (ImprovedVideoCompressor._parse_inter); the byte fields are views of the payload."""
+    __slots__ = ("v1", "h", "w", "isz", "ch", "raw", "k", "l", "wlen", "ones", "mask_bytes", "witness_bytes", "vcount", "vz")
+
+
+class _InterJob:
+    """An inter frame on its way through decompress_video: the parsed payload (or its parse error) and its inflates."""
+    __slots__ = ("p", "err", "values", "mask", "values_arr", "mask_arr", "l", "wlen")
+
+    def __init__(self):
+        self.p = self.err = self.values = self.mask = self.values_arr = self.mask_arr = None
+        self.l = self.wlen = 0
+
+
 class ImprovedVideoCompressor:
     """ivc.ImprovedVideoCompressor (ivc:309-523) with the GOP loop wired in.
 
@@ -408,6 +422,26 @@ class ImprovedVideoCompressor:
             body += struct.pack("<I", nb) + bm_row[:nb].tobytes() + struct.pack("<I", nw) + wt_row[:nw].tobytes()
         body += struct.pack("<II", len(vz), vcount) + vz
         return hdr + body
+
+    @staticmethod
+    def _parse_inter(payload: bytes) -> "_InterPayload":
+        """The fields of an inter-frame payload (the inverse of _inter_layout; also reads round 1's 'RBF1' tag, whose raw masks are
+        plain np.packbits bytes).  Nothing is decompressed: `mask_bytes` is the stored raw mask or bitmap, `vz` the value stream."""
+        p = _InterPayload()
+        p.v1 = payload[:len(_INTER_TAG_V1)] == _INTER_TAG_V1
+        mv = memoryview(payload)
+        pos = len(_INTER_TAG)
+        p.h, p.w, p.isz, p.ch, p.raw = struct.unpack_from("<IIIBB", payload, pos)
+        pos += struct.calcsize("<IIIBB")
+        p.k, p.l, p.wlen, p.ones = struct.unpack_from("<dIIQ", payload, pos)
+        pos += struct.calcsize("<dIIQ")
+        (bl,) = struct.unpack_from("<I", payload, pos); pos += 4
+        p.mask_bytes = mv[pos:pos + bl]; pos += bl
+        (wl,) = struct.unpack_from("<I", payload, pos); pos += 4
+        p.witness_bytes = mv[pos:pos + wl]; pos += wl
+        vlen, p.vcount = struct.unpack_from("<II", payload, pos); pos += 8
+        p.vz = mv[pos:pos + vlen]
+        return p
 
     def _encode_inter_frames(self, datas: List[np.ndarray], inter: List[int], pool) -> Dict[int, object]:
         """Futures of the inter-frame payloads for frame indices `inter` (each coded against frame i-1); None = keyframe instead."""
@@ -523,55 +557,109 @@ class ImprovedVideoCompressor:
         return results
 
     # ------------------------------------------------------------------ decode
-    def _decode_inter(self, payload: bytes, prev):
-        v1 = payload[:len(_INTER_TAG_V1)] == _INTER_TAG_V1
-        pos = len(_INTER_TAG)
-        h, w, isz, ch, raw = struct.unpack_from("<IIIBB", payload, pos)
-        pos += struct.calcsize("<IIIBB")
-        k, l, wlen, ones = struct.unpack_from("<dIIQ", payload, pos)
-        pos += struct.calcsize("<dIIQ")
-        (bl,) = struct.unpack_from("<I", payload, pos); pos += 4
-        bbytes = np.frombuffer(payload, dtype=np.uint8, count=bl, offset=pos); pos += bl
-        (wl,) = struct.unpack_from("<I", payload, pos); pos += 4
-        wbytes = np.frombuffer(payload, dtype=np.uint8, count=wl, offset=pos); pos += wl
-        vlen, vcount = struct.unpack_from("<II", payload, pos); pos += 8
-        dtype = np.uint8 if isz == 1 else np.uint16
-        values = np.frombuffer(zlib.decompress(payload[pos:pos + vlen]), dtype=dtype)[:vcount]
-        n = h * w
-        pdata = _frame_data(prev)
-        exp_shape = (h, w, ch) if ch > 1 else (h, w)
-        if pdata.shape != exp_shape or pdata.dtype != np.dtype(dtype):
-            raise ValueError(f"inter frame {exp_shape}/{np.dtype(dtype)} does not match the previous frame {pdata.shape}/{pdata.dtype}")
-        if values.size != ones * ch:
-            raise ValueError(f"corrupt inter frame: {values.size} changed values for {ones} changed pixels x {ch} channels")
-        if raw:
-            rbits = bbytes if v1 else np.frombuffer(zlib.decompress(bbytes.tobytes()), dtype=np.uint8)
-            mask = np.unpackbits(rbits)[:n]
-        else:
-            bitmap = np.unpackbits(bbytes)[:l]
-            witness = np.unpackbits(wbytes)[:wlen]
-            mask = BloomFilterCompressor().decompress(bitmap, witness, n, k)
-        st = getattr(self, "_dec_stream", None)
-        if st is None or (st.H, st.W, st.C, st.dtype) != (h, w, ch, np.dtype(dtype)):
-            st = FrameStream(h, w, ch, dtype, max_frames=2, max_pairs=1, k1_only=True)
-            self._dec_stream, self._dec_slot, self._dec_src = st, 0, None
-        if self._dec_src is not prev:                             # previous frame is not the one resident on the device
-            st.upload(np.ascontiguousarray(pdata)[None], first=0)
-            self._dec_slot = 0
-        nxt_slot = 1 - self._dec_slot
-        applied = st.apply_diff(self._dec_slot, nxt_slot, mask, values)     # N2: scatter on the device
-        if applied != ones:                                       # the reference would silently return the base frame (ivc:882)
-            self._dec_src = None
-            raise ValueError(f"corrupt inter frame: the decoded mask selects {int(np.count_nonzero(mask))} pixels, the payload "
-                             f"announces {ones}")
-        out = st.download(nxt_slot)
-        self._dec_slot = nxt_slot
-        res = YUVFrame(out) if hasattr(prev, "yuv_info") else out
-        self._dec_src = res
-        return res
+    def _start_inter(self, payload: bytes, pool) -> "_InterJob":
+        """Parse an inter payload and start its inflates (changed values, zlib'd raw mask) in `pool`.  A parse error is kept and
+        raised when decoding reaches this frame, so the first bad frame of the file decides the exception."""
+        job = _InterJob()
+        try:
+            job.p = self._parse_inter(payload)
+        except Exception as e:                               # re-raised in file order by _check_inter
+            job.err = e
+            return job
+        job.values = pool.submit(zlib.decompress, job.p.vz)
+        if job.p.raw and not job.p.v1:
+            job.mask = pool.submit(zlib.decompress, job.p.mask_bytes)
+        return job
+
+    @staticmethod
+    def _check_inter(job: "_InterJob", pdata: np.ndarray) -> None:
+        """The checks of one inter frame that need no GPU, in the order a frame-by-frame decode makes them; keeps the inflated
+        values and the effective mask fields on `job`."""
+        if job.err is not None:
+            raise job.err
+        p = job.p
+        dtype = np.dtype(np.uint8 if p.isz == 1 else np.uint16)
+        job.values_arr = np.frombuffer(job.values.result(), dtype=dtype)[:p.vcount]
+        exp_shape = (p.h, p.w, p.ch) if p.ch > 1 else (p.h, p.w)
+        if pdata.shape != exp_shape or pdata.dtype != dtype:
+            raise ValueError(f"inter frame {exp_shape}/{dtype} does not match the previous frame {pdata.shape}/{pdata.dtype}")
+        if job.values_arr.size != p.ones * p.ch:
+            raise ValueError(f"corrupt inter frame: {job.values_arr.size} changed values for {p.ones} changed pixels x {p.ch} channels")
+        if p.raw:
+            job.mask_arr = np.frombuffer(p.mask_bytes if p.v1 else job.mask.result(), dtype=np.uint8)
+            if job.mask_arr.size < (p.h * p.w + 7) // 8:
+                raise ValueError(f"corrupt inter frame: the raw mask holds {8 * job.mask_arr.size} of {p.h * p.w} bits")
+            return
+        job.l = min(p.l, 8 * len(p.mask_bytes))              # the bits that are there, as np.unpackbits(..)[:l] keeps them
+        job.wlen = min(p.wlen, 8 * len(p.witness_bytes))
+        if job.l == 0 or job.wlen == 0:                      # the reference would take the l-bit bitmap as the n-bit mask (ivc:282-284)
+            raise ValueError(f"corrupt inter frame: a coded mask with {job.l} Bloom bits and {job.wlen} witness bits")
+        if not p.k >= 0.0:
+            raise _cabi.RbfError(f"corrupt inter frame: k = {p.k}")
+
+    @staticmethod
+    def _decode_group(st: FrameStream, base: int, group: List["_InterJob"]) -> np.ndarray:
+        """Frames base+1 .. base+len(group) of `st` (slots modulo st.max_frames) from frame `base` and the group's payloads: one
+        decode_masks, one apply_chain and one download_batch.  Raises the first bad frame's error."""
+        m, n = len(group), st.npix
+        raws = [bool(j.p.raw) for j in group]
+        nbs = [(n + 7) // 8 if r else (j.l + 7) // 8 for j, r in zip(group, raws)]
+        nws = [0 if r else (j.wlen + 7) // 8 for j, r in zip(group, raws)]
+        bms = np.zeros((m, max(16, (max(nbs) + 15) // 16 * 16)), dtype=np.uint8)
+        wts = np.zeros((m, 0 if not any(nws) else max(16, (max(nws) + 15) // 16 * 16)), dtype=np.uint8)
+        for i, j in enumerate(group):
+            if raws[i]:
+                bms[i, :nbs[i]] = j.mask_arr[:nbs[i]]
+            else:
+                bms[i, :nbs[i]] = np.frombuffer(j.p.mask_bytes, dtype=np.uint8, count=nbs[i])
+                wts[i, :nws[i]] = np.frombuffer(j.p.witness_bytes, dtype=np.uint8, count=nws[i])
+        consumed, ones = st.decode_masks(bms, wts, [0 if r else j.l for j, r in zip(group, raws)],
+                                         [0 if r else j.wlen for j, r in zip(group, raws)], [j.p.k for j in group], raws)
+        for i, j in enumerate(group):
+            if not raws[i] and consumed[i] > j.wlen:         # the reference's witness[witness_idx] raises here
+                raise IndexError("list index out of range")
+            if ones[i] != j.p.ones:                          # the reference would silently return the base frame (ivc:882)
+                raise ValueError(f"corrupt inter frame: the decoded mask selects {int(ones[i])} pixels, the payload announces {j.p.ones}")
+        applied = st.apply_chain(base, [j.values_arr for j in group])
+        if not np.array_equal(applied, ones):
+            raise ValueError(f"corrupt inter frame: {applied.tolist()} pixels applied, {ones.tolist()} expected")
+        return st.download_batch((base + 1) % st.max_frames, m)
+
+    def _decode_run(self, run: List["_InterJob"], prev, streams: Dict[tuple, FrameStream]) -> list:
+        """The frames of a run of consecutive inter payloads that follows `prev`, in groups of batch_size.  The run's base frame is
+        uploaded once; each group chains from the previous group's last frame, which stays on the device."""
+        pdata = np.ascontiguousarray(_frame_data(prev))
+        group_size = max(1, int(self.batch_size))
+        out, st, base = [], None, 0
+        for g0 in range(0, len(run), group_size):
+            group, err = [], None
+            for job in run[g0:g0 + group_size]:
+                try:
+                    self._check_inter(job, pdata)
+                except Exception as e:                       # the frames before it are decoded first: their errors come first
+                    err = e
+                    break
+                group.append(job)
+            if group:
+                if st is None:
+                    ch = pdata.shape[2] if pdata.ndim == 3 else 1
+                    key = (pdata.shape, pdata.dtype.str)
+                    st = streams.get(key)
+                    if st is None:
+                        st = streams[key] = FrameStream(pdata.shape[0], pdata.shape[1], ch, pdata.dtype, max_frames=group_size + 1,
+                                                        max_pairs=group_size, k1_only=True)
+                    st.upload(pdata, first=0)
+                dec = self._decode_group(st, base, group)
+                base = (base + len(group)) % st.max_frames
+                out += [YUVFrame(f) if hasattr(prev, "yuv_info") else f for f in dec]
+            if err is not None:
+                raise err
+        return out
 
     def decompress_video(self, input_path: str = None, output_path: Optional[str] = None,
                          compressed_frames: List[bytes] = None, metadata: Dict = None) -> List[np.ndarray]:
+        """ivc:452-504.  Every zlib stream (keyframe blobs, changed values, raw masks) is inflated in a pool of num_threads; each
+        run of inter frames is rebuilt on the GPU in groups of batch_size (_decode_run)."""
         if input_path and os.path.exists(input_path):                              # ivc:471-485
             with open(input_path, "rb") as fh:
                 magic = fh.read(4)
@@ -584,14 +672,30 @@ class ImprovedVideoCompressor:
                     compressed_frames.append(fh.read(size))
         if not compressed_frames:
             raise ValueError("No compressed frames provided")                       # ivc:487-488
-        frames = []
-        for c in compressed_frames:
-            if c[:len(_INTER_TAG)] in (_INTER_TAG, _INTER_TAG_V1):
+        from concurrent.futures import ThreadPoolExecutor
+        frames: list = []
+        streams: Dict[tuple, FrameStream] = {}
+        pool = ThreadPoolExecutor(self.num_threads)
+        try:
+            jobs = [self._start_inter(c, pool) if c[:len(_INTER_TAG)] in (_INTER_TAG, _INTER_TAG_V1)
+                    else pool.submit(self.compressor.decompress_frame, c) for c in compressed_frames]
+            i = 0
+            while i < len(jobs):
+                if not isinstance(jobs[i], _InterJob):
+                    frames.append(jobs[i].result())
+                    i += 1
+                    continue
                 if not frames:
                     raise ValueError("inter frame without a preceding frame")
-                frames.append(self._decode_inter(c, frames[-1]))
-            else:
-                frames.append(self.compressor.decompress_frame(c))
+                j = i
+                while j < len(jobs) and isinstance(jobs[j], _InterJob):
+                    j += 1
+                frames += self._decode_run(jobs[i:j], frames[-1], streams)
+                i = j
+        finally:
+            pool.shutdown(wait=True, cancel_futures=True)
+            for st in streams.values():
+                st.close()
         if output_path:
             self.save_frames_as_video(frames, output_path)
         return frames

@@ -178,6 +178,49 @@ class FrameStream:
         _cabi.check(_cabi.lib().rbf_stream_download(self._h, int(frame), _cabi.ptr(out)), _cabi.ctx())
         return out
 
+    # ------------------------------------------------------------------ batched decode (K4b / K4c)
+    def decode_masks(self, bitmaps: np.ndarray, witnesses: np.ndarray, l, wlen, k, raw, seeds=_cabi.IVC_SEEDS):
+        """BloomFilterCompressor.decompress (ivc:268-307) of a group of pairs in one launch; the masks land in mask slots 0..count-1.
+        bitmaps uint8[count, bslot]: row i holds np.packbits of pair i's l-bit array, or of its n-bit mask when raw[i];
+        witnesses uint8[count, wslot] (wslot may be 0 when every pair is raw).  Bytes past a row's payload are ignored.
+        -> (consumed uint64[count]: positions that passed the Bloom test, ones uint64[count]: set bits of each decoded mask)."""
+        bm = np.ascontiguousarray(bitmaps, dtype=np.uint8)
+        wt = np.ascontiguousarray(witnesses, dtype=np.uint8)
+        count = bm.shape[0]
+        ls, ws = np.ascontiguousarray(l, dtype=np.uint64), np.ascontiguousarray(wlen, dtype=np.uint64)
+        ks, rs = np.ascontiguousarray(k, dtype=np.float64), np.ascontiguousarray(raw, dtype=np.uint8)
+        if wt.shape[0] != count or not (ls.size == ws.size == ks.size == rs.size == count):
+            raise ValueError("one bitmap, witness, l, wlen, k and raw flag per pair")
+        consumed = np.zeros(count, dtype=np.uint64)
+        ones = np.zeros(count, dtype=np.uint64)
+        sd = _cabi.seeds_struct(seeds)
+        wslot = wt.shape[1] if wt.ndim == 2 else 0
+        _cabi.check(_cabi.lib().rbf_stream_decode_masks(self._h, count, _cabi.ptr(bm), bm.shape[1], _cabi.ptr(wt) if wslot else None,
+                                                        wslot, _cabi.ptr(ls), _cabi.ptr(ws), _cabi.ptr(ks), _cabi.ptr(rs),
+                                                        C.byref(sd), _cabi.ptr(consumed), _cabi.ptr(ones)), _cabi.ctx())
+        self.pairs = 0
+        return consumed, ones
+
+    def apply_chain(self, base_frame: int, values: Sequence[np.ndarray]) -> np.ndarray:
+        """Frame base_frame+1+i = frame base_frame+i with mask slot i applied, values[i] replacing its set pixels in rank order
+        (ivc:849-909), for i < len(values); slots are taken modulo max_frames.  -> uint64[count] pixels applied per pair: 0 from
+        the first pair whose value count does not match its mask (ivc:882), whose frame and every later one are not written."""
+        parts = [memoryview(np.ascontiguousarray(v)).cast("B") for v in values]
+        offs = np.zeros(len(parts) + 1, dtype=np.uint64)
+        offs[1:] = np.cumsum([p.nbytes for p in parts])
+        buf = np.frombuffer(b"".join(parts), dtype=np.uint8)
+        applied = np.zeros(len(parts), dtype=np.uint64)
+        _cabi.check(_cabi.lib().rbf_stream_apply_chain(self._h, int(base_frame), len(parts), _cabi.ptr(buf) if buf.size else None,
+                                                       _cabi.ptr(offs), _cabi.ptr(applied)), _cabi.ctx())
+        return applied
+
+    def download_batch(self, first: int, count: int) -> np.ndarray:
+        """Frames first .. first+count-1 (slots modulo max_frames) -> [count, H, W(, C)], one copy and one synchronisation."""
+        shape = (int(count), self.H, self.W, self.C) if self.C > 1 else (int(count), self.H, self.W)
+        out = np.empty(shape, dtype=self.dtype)
+        _cabi.check(_cabi.lib().rbf_stream_download_batch(self._h, int(first), int(count), _cabi.ptr(out)), _cabi.ctx())
+        return out
+
     def stage_ms(self) -> dict:
         out = (C.c_double * 6)()
         _cabi.check(_cabi.lib().rbf_stream_stage_ms(self._h, out), _cabi.ctx())
