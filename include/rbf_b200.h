@@ -147,7 +147,10 @@ void rbf_stream_destroy(rbf_stream* s);
  *               infos report wlen = 0 and rbf_stream_fetch refuses bitmap / witness pointers
  *   "mask_mode" 0: |dY| > threshold (ivc:808); 1: additionally any byte of the pixel differs (lossless GOP mode)
  *   "gray_mode" 1: 3-channel frames are BGR and the mask is taken on cv2.cvtColor(.., COLOR_BGR2GRAY) (ivc:792-795),
- *               OpenCV's fixed point (3735 B + 19235 G + 9798 R + 16384) >> 15 for 8- and 16-bit samples */
+ *               OpenCV's fixed point (3735 B + 19235 G + 9798 R + 16384) >> 15 for 8- and 16-bit samples
+ *   "value_mode" what rbf_stream_gather_changed and rbf_stream_zlib_changed return per changed pixel: 0 (default) the current
+ *               frame's samples; 1 residuals (curr - prev) mod 2^(8 sample_bytes) per sample, little-endian, in the same order
+ *               and count.  1 needs 1 or 3 channels of 1- or 2-byte samples; other values or shapes are RBF_ERR_INVALID */
 int rbf_stream_set_option(rbf_stream* s, const char* key, int64_t value);
 int rbf_stream_upload(rbf_stream* s, uint32_t first_frame, uint32_t count, const void* host_frames);
 int rbf_stream_frame_ptr(rbf_stream* s, uint32_t frame, void** dptr);
@@ -205,6 +208,11 @@ int rbf_stream_download(rbf_stream* s, uint32_t frame, void* host_out);
  *     are taken modulo max_frames, so a chain may continue from the last frame of the previous one wherever it sits; count <
  *     max_frames.  ivc:882 per pair: pair i is applied only if its mask's popcount x pixel bytes equals its value bytes; the
  *     first pair that fails gets applied_out[i] = 0 and no frame from there on is written.  applied_out[i] = pixels applied.
+ * rbf_stream_apply_chain_modes  rbf_stream_apply_chain with a coding per pair: residual[i] == 1 means pair i's values are
+ *     residuals (what a gather with value_mode 1 returns), added to the selected pixels per sample mod 2^(8 sample_bytes) instead
+ *     of replacing them; 0 means plain values.  residual may be NULL (every pair plain: rbf_stream_apply_chain itself); a flag
+ *     other than 0 or 1 is RBF_ERR_INVALID.  The flags travel in the same H2D copy as the offsets; ivc:882, the first-bad-pair
+ *     rule and slot wrap-around are the same for both kinds.
  * rbf_stream_download_batch  frames first .. first+count-1 (slots modulo max_frames) into one contiguous host array, one
  *     synchronisation. */
 int rbf_stream_decode_masks(rbf_stream* s, uint32_t count, const uint8_t* bitmaps_packbits, uint64_t bitmap_slot_bytes,
@@ -212,6 +220,8 @@ int rbf_stream_decode_masks(rbf_stream* s, uint32_t count, const uint8_t* bitmap
                             const double* k, const uint8_t* raw, const rbf_seeds* seeds, uint64_t* consumed_out, uint64_t* ones_out);
 int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values, const uint64_t* value_offsets,
                            uint64_t* applied_out);
+int rbf_stream_apply_chain_modes(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
+                                 const uint64_t* value_offsets, const uint8_t* residual /* [count] or NULL */, uint64_t* applied_out);
 int rbf_stream_download_batch(rbf_stream* s, uint32_t first, uint32_t count, void* host_out);
 /* N3  the 5x5 median of cv2.medianBlur in VideoFrameCompressor._estimate_noise_level (ivc:738): replicated border, 13th
  *     smallest of 25, exact for uint8 / uint16.  The float32 std of (frame - median) stays in numpy (ivc:741-744). */

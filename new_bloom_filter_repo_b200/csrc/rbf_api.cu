@@ -596,6 +596,7 @@ struct rbf_stream {
     int k1_only = 0;        // stop after K1 (mask + counts): VideoFrameCompressor._calculate_frame_diff
     int mask_mode = 0;      // 0: |dY| > thr (ivc:808); 1: additionally any byte of the pixel differs
     int gray_mode = 0;      // 1: the mask is taken on cv2.COLOR_BGR2GRAY of the pixel (ivc:792-795) instead of on sample 0
+    int value_mode = 0;     // changed-value gathers: 0 the current samples; 1 residuals (curr - prev) mod 2^(8 S) per sample
     bool last_k1_only = false;
     size_t bits_hwm = 0, wit_hwm = 0;   // bytes per slot that may hold set bits (see stream_clear_outputs)
     bool wit_dirty_full = false;
@@ -671,6 +672,13 @@ extern "C" int rbf_stream_set_option(rbf_stream* s, const char* key, int64_t v) 
     if (!strcmp(key, "gray_mode")) {
         if (v && s->C != 3) return set_err(s->c, RBF_ERR_INVALID, "gray_mode needs 3-channel frames");
         s->gray_mode = v ? 1 : 0;
+        return RBF_OK;
+    }
+    if (!strcmp(key, "value_mode")) {
+        if (v != 0 && v != 1) return set_err(s->c, RBF_ERR_INVALID, "value_mode must be 0 (values) or 1 (residuals), not %lld", (long long)v);
+        if (v && !((s->C == 1 || s->C == 3) && (s->S == 1 || s->S == 2)))
+            return set_err(s->c, RBF_ERR_INVALID, "residual values need 1 or 3 channels of 8- or 16-bit samples (C=%u S=%u)", s->C, s->S);
+        s->value_mode = (int)v;
         return RBF_OK;
     }
     return set_err(s->c, RBF_ERR_INVALID, "unknown stream option %s", key);
@@ -1172,13 +1180,15 @@ extern "C" int rbf_stream_gather_changed(rbf_stream* s, uint32_t pairs, uint8_t*
     for (uint32_t i = 0; i < pairs; i++) {
         jobs[i].mask = s->d_mask + (size_t)i * s->mask_stride_w;
         jobs[i].frame = s->h_pairs[i].curr;
+        jobs[i].prev = s->h_pairs[i].prev;
         jobs[i].values = (uint8_t*)d_vals + offsets_out[i];
         jobs[i].out_frame = nullptr;
         jobs[i].npix = (uint32_t)s->npix;
         jobs[i].pix_bytes = (uint32_t)pb;
     }
     CK(c, cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(GatherJob) * pairs, cudaMemcpyHostToDevice, c->st));
-    LAUNCH(c, launch_gather_scatter((const GatherJob*)d_jobs, (int)pairs, 0, (uint32_t)s->npix, (uint32_t)pb, (uint32_t*)d_gcnt, nullptr, c->st));
+    LAUNCH(c, launch_gather_scatter((const GatherJob*)d_jobs, (int)pairs, 0, (uint32_t)s->npix, (uint32_t)pb, (uint32_t*)d_gcnt, nullptr, c->st,
+                                    s->value_mode ? s->S : 0u));
     c->launches++;
     if (total) { CK(c, cudaMemcpyAsync(values_out, d_vals, (size_t)total, cudaMemcpyDeviceToHost, c->st)); c->d2h += (int64_t)total; }
     CK(c, cudaStreamSynchronize(c->st));
@@ -1318,6 +1328,11 @@ extern "C" int rbf_stream_decode_masks(rbf_stream* s, uint32_t count, const uint
 
 extern "C" int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
                                       const uint64_t* value_offsets, uint64_t* applied_out) {
+    return rbf_stream_apply_chain_modes(s, base_frame, count, values, value_offsets, nullptr, applied_out);
+}
+
+extern "C" int rbf_stream_apply_chain_modes(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
+                                            const uint64_t* value_offsets, const uint8_t* residual, uint64_t* applied_out) {
     if (!s || !value_offsets || !applied_out) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_apply_chain: NULL");
     rbf_ctx* c = s->c;
     if (count == 0 || count > s->max_pairs || count >= s->max_frames || base_frame >= s->max_frames)
@@ -1325,21 +1340,35 @@ extern "C" int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32
                        base_frame, s->max_frames, s->max_pairs);
     for (uint32_t i = 0; i < count; i++)
         if (value_offsets[i + 1] < value_offsets[i]) return set_err(c, RBF_ERR_INVALID, "value offsets decrease at pair %u", i);
+    bool any_residual = false;
+    for (uint32_t i = 0; residual && i < count; i++) {
+        if (residual[i] > 1) return set_err(c, RBF_ERR_INVALID, "pair %u: residual flag %u is neither 0 nor 1", i, (unsigned)residual[i]);
+        any_residual |= residual[i] != 0;
+    }
     const uint64_t vbytes = value_offsets[count];
     if (vbytes && !values) return set_err(c, RBF_ERR_INVALID, "rbf_stream_apply_chain: values is NULL");
     CK(c, cudaSetDevice(c->device));
     const uint32_t ntiles = (uint32_t)((s->npix + AP_TILE_PX - 1) / AP_TILE_PX);
     void *d_vals, *d_small, *d_pfx;
     int rc;
-    const size_t small = align_up(8 * ((size_t)count + 1), 16) + 4 * ((size_t)count + 1);
+    // d_small: the value offsets, then the residual flags (one H2D copy for both), then first_bad and the totals
+    const size_t off_bytes = 8 * ((size_t)count + 1), flag_bytes = residual ? count : 0, res_at = align_up(off_bytes + flag_bytes, 16);
+    const size_t small = res_at + 4 * ((size_t)count + 1);
     if ((rc = scratch_get(c, 8, (size_t)vbytes + 256, &d_vals)) || (rc = scratch_get(c, 22, small, &d_small)) ||
         (rc = scratch_get(c, 23, 4 * (size_t)count * ntiles, &d_pfx)))
         return rc;
     uint64_t* d_off = (uint64_t*)d_small;
-    uint32_t* d_res = (uint32_t*)((uint8_t*)d_small + align_up(8 * ((size_t)count + 1), 16));   // [0] first_bad, [1 + i] totals
+    uint32_t* d_res = (uint32_t*)((uint8_t*)d_small + res_at);   // [0] first_bad, [1 + i] totals
     if (vbytes) { CK(c, cudaMemcpyAsync(d_vals, values, (size_t)vbytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)vbytes; }
-    CK(c, cudaMemcpyAsync(d_off, value_offsets, 8 * ((size_t)count + 1), cudaMemcpyHostToDevice, c->st));
-    c->h2d += 8 * ((int64_t)count + 1);
+    if (residual) {
+        std::vector<uint8_t> head(off_bytes + flag_bytes);
+        memcpy(head.data(), value_offsets, off_bytes);
+        memcpy(head.data() + off_bytes, residual, flag_bytes);
+        CK(c, cudaMemcpyAsync(d_off, head.data(), head.size(), cudaMemcpyHostToDevice, c->st));   // pageable: staged before return
+    } else {
+        CK(c, cudaMemcpyAsync(d_off, value_offsets, off_bytes, cudaMemcpyHostToDevice, c->st));
+    }
+    c->h2d += (int64_t)(off_bytes + flag_bytes);
     CK(c, cudaMemsetAsync(d_res, 0xff, 4, c->st));
     ApplyChain A;
     A.masks = s->d_mask; A.mask_stride_w = s->mask_stride_w;
@@ -1347,6 +1376,8 @@ extern "C" int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32
     A.max_frames = s->max_frames; A.base = base_frame;
     A.npix = (uint32_t)s->npix; A.ntiles = ntiles; A.count = count; A.pix_bytes = s->C * s->S;
     A.values = (const uint8_t*)d_vals; A.value_off = d_off;
+    A.residual = any_residual ? (const uint8_t*)d_small + off_bytes : nullptr;   // a group without residual pairs runs the plain sweep
+    A.sample_bytes = s->S;
     A.tile_pfx = (uint32_t*)d_pfx; A.totals = d_res + 1; A.first_bad = d_res;
     LAUNCH(c, launch_apply_chain(A, c->sm_count, c->st));
     c->launches += 2;                                   // tile count + tile scan
@@ -1541,6 +1572,7 @@ extern "C" int rbf_stream_zlib_changed(rbf_stream* s, uint32_t pairs, uint8_t* o
     for (uint32_t i = 0; i < pairs; i++) {
         jobs[i].mask = s->d_mask + (size_t)i * s->mask_stride_w;
         jobs[i].frame = s->h_pairs[i].curr;
+        jobs[i].prev = s->h_pairs[i].prev;
         jobs[i].values = (uint8_t*)d_vals + voff[i];
         jobs[i].out_frame = nullptr;
         jobs[i].npix = (uint32_t)s->npix;
@@ -1549,7 +1581,8 @@ extern "C" int rbf_stream_zlib_changed(rbf_stream* s, uint32_t pairs, uint8_t* o
         lens[i] = voff[i + 1] - voff[i];
     }
     CK(c, cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(GatherJob) * pairs, cudaMemcpyHostToDevice, c->st));
-    LAUNCH(c, launch_gather_scatter((const GatherJob*)d_jobs, (int)pairs, 0, (uint32_t)s->npix, (uint32_t)pb, (uint32_t*)d_gcnt, nullptr, c->st));
+    LAUNCH(c, launch_gather_scatter((const GatherJob*)d_jobs, (int)pairs, 0, (uint32_t)s->npix, (uint32_t)pb, (uint32_t*)d_gcnt, nullptr, c->st,
+                                    s->value_mode ? s->S : 0u));
     c->launches++;
     return zlib_batch(c, pairs, srcs.data(), lens.data(), true, out_host, out_capacity, out_offsets);   // same stream: after the gather
 }

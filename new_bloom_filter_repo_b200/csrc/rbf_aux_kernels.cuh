@@ -39,7 +39,36 @@ __device__ __forceinline__ void copy_pixel(uint8_t* __restrict__ dst, const uint
     for (int q = 0; q < PB; q++) dst[q] = src[q];          // PB = 1 or 3: all loads first, then the stores
 }
 
-template <int PB>
+// Residual coding of the value streams: per sample of S bytes (1, or 2 little-endian), dst = (curr - prev) mod 2^(8S) on the encode
+// side and dst = (dst + r) mod 2^(8S) on the decode side.  PB = channels x S; the pair (PB, S) is one of (1,1), (3,1), (2,2), (6,2).
+template <int PB, int S>
+__device__ __forceinline__ void resid_pixel(uint8_t* __restrict__ dst, const uint8_t* __restrict__ curr, const uint8_t* __restrict__ prev) {
+    static_assert((S == 1 || S == 2) && PB % S == 0, "sample bytes");
+    if constexpr (S == 2) {
+#pragma unroll
+        for (int q = 0; q < PB / 2; q++)
+            reinterpret_cast<uint16_t*>(dst)[q] = (uint16_t)(reinterpret_cast<const uint16_t*>(curr)[q] - reinterpret_cast<const uint16_t*>(prev)[q]);
+    } else {
+#pragma unroll
+        for (int q = 0; q < PB; q++) dst[q] = (uint8_t)(curr[q] - prev[q]);
+    }
+}
+
+template <int PB, int S>
+__device__ __forceinline__ void add_pixel(uint8_t* __restrict__ dst, const uint8_t* __restrict__ r) {
+    static_assert((S == 1 || S == 2) && PB % S == 0, "sample bytes");
+    if constexpr (S == 2) {
+#pragma unroll
+        for (int q = 0; q < PB / 2; q++)
+            reinterpret_cast<uint16_t*>(dst)[q] = (uint16_t)(reinterpret_cast<uint16_t*>(dst)[q] + reinterpret_cast<const uint16_t*>(r)[q]);
+    } else {
+#pragma unroll
+        for (int q = 0; q < PB; q++) dst[q] = (uint8_t)(dst[q] + r[q]);
+    }
+}
+
+// RS = 0: plain gather / scatter of the pixels; RS = 1 or 2: the gather stores residuals against J.prev per sample of RS bytes
+template <int PB, int RS>
 __global__ void __launch_bounds__(1024) k_gather_scatter(const GatherJob* __restrict__ jobs, int scatter, uint32_t chunks,
                                                           const uint32_t* __restrict__ counts, uint32_t* __restrict__ totals) {
     const GatherJob J = jobs[blockIdx.y];
@@ -57,7 +86,8 @@ __global__ void __launch_bounds__(1024) k_gather_scatter(const GatherJob* __rest
             const uint32_t b = __ffs(m) - 1;
             m &= m - 1u;
             const size_t px = ((size_t)w << 5) + b;
-            if (scatter) copy_pixel<PB>(J.out_frame + px * PB, J.values + (size_t)rank * PB);
+            if constexpr (RS != 0) resid_pixel<PB, RS>(J.values + (size_t)rank * PB, J.frame + px * PB, J.prev + px * PB);
+            else if (scatter) copy_pixel<PB>(J.out_frame + px * PB, J.values + (size_t)rank * PB);
             else copy_pixel<PB>(J.values + (size_t)rank * PB, J.frame + px * PB);
             rank++;
         }

@@ -35,7 +35,8 @@ __global__ void __launch_bounds__(256) k_mask_popcount(const uint32_t* __restric
 // pair, one CTA per pair), which also checks ivc:882 -- popcount x pixel bytes == the pair's value bytes -- and records the first
 // pair that fails.  k_apply_sweep then runs persistent CTAs that each own a share of the tiles: the base frame's tile is loaded
 // into shared memory once and walked through the chain -- replace the set pixels of mask t in rank order, store the tile as
-// output frame t with 16 B stores -- for every t before the first failing pair.  Each output frame is written once and nothing
+// output frame t with 16 B stores -- for every t before the first failing pair.  A residual pair adds its values to the set
+// pixels per sample instead of replacing them (value_mode 1 of the gather).  Each output frame is written once and nothing
 // is copied device to device.  Frame slots are taken modulo max_frames, so a chain continues from the last frame of the
 // previous one wherever it sits.
 // Ragged end: the last tile of a frame is loaded and stored as whole 16 B units plus single bytes for the rest (frames start
@@ -79,7 +80,9 @@ __global__ void __launch_bounds__(1024) k_tile_scan(const ApplyChain A) {
     }
 }
 
-template <int PB>
+// RS = 0: every pair is plain (A.residual is not read).  RS = 1 or 2: pairs with A.residual[t] set add their values to the tile per
+// sample of RS bytes, with wrap-around; the other pairs replace pixels as in the plain sweep.
+template <int PB, int RS>
 __global__ void __launch_bounds__(AP_THREADS) k_apply_sweep(const ApplyChain A) {
     __shared__ __align__(16) uint8_t tile[AP_TILE_PX * PB];
     __shared__ uint32_t s_warp[33];
@@ -105,10 +108,17 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply_sweep(const ApplyChain A) 
             // its barriers also order the previous iteration's stores (and the load above) before this iteration's writes
             const uint32_t rank = pfx + block_excl_scan(__popc(m), s_warp, tot);
             const uint8_t* v = A.values + A.value_off[t] + (size_t)rank * PB;
+            bool add = false;
+            if constexpr (RS != 0) add = __ldg(A.residual + t) != 0;
             while (m) {
                 const uint32_t b = __ffs(m) - 1;
                 m &= m - 1u;
-                copy_pixel<PB>(tile + (threadIdx.x * 32u + b) * PB, v);
+                if constexpr (RS != 0) {
+                    if (add) add_pixel<PB, RS>(tile + (threadIdx.x * 32u + b) * PB, v);
+                    else copy_pixel<PB>(tile + (threadIdx.x * 32u + b) * PB, v);
+                } else {
+                    copy_pixel<PB>(tile + (threadIdx.x * 32u + b) * PB, v);
+                }
                 v += PB;
             }
             __syncthreads();

@@ -380,16 +380,24 @@ uint32_t gather_chunks(uint32_t npix) {
 }
 // d_counts: F * gather_chunks(npix) uint32 of scratch; d_totals (may be NULL): set pixels per pair
 cudaError_t launch_gather_scatter(const GatherJob* d_jobs, int F, int scatter, uint32_t npix, uint32_t pix_bytes, uint32_t* d_counts,
-                                  uint32_t* d_totals, cudaStream_t st) {
+                                  uint32_t* d_totals, cudaStream_t st, uint32_t resid_sample_bytes) {
     if (F <= 0) return cudaSuccess;
+    // the kernel is picked by (pixel bytes, residual sample bytes): 2 B per pixel is one 16-bit sample, never two 8-bit ones
+    const uint32_t key = pix_bytes * 4u + resid_sample_bytes;
+    if (resid_sample_bytes && (scatter || !(key == 1u * 4 + 1 || key == 3u * 4 + 1 || key == 2u * 4 + 2 || key == 6u * 4 + 2)))
+        return cudaErrorInvalidValue;                                 // checked before anything is launched
     const uint32_t ch = gather_chunks(npix);
     const dim3 grid(ch, (unsigned)F);
     k_mask_chunk_count<<<grid, 256, 0, st>>>(d_jobs, ch, d_counts);
-    switch (pix_bytes) {
-    case 1: k_gather_scatter<1><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
-    case 2: k_gather_scatter<2><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
-    case 3: k_gather_scatter<3><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
-    case 6: k_gather_scatter<6><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
+    switch (key) {
+    case 1u * 4: k_gather_scatter<1, 0><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
+    case 2u * 4: k_gather_scatter<2, 0><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
+    case 3u * 4: k_gather_scatter<3, 0><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
+    case 6u * 4: k_gather_scatter<6, 0><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
+    case 1u * 4 + 1: k_gather_scatter<1, 1><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;   // 1 x 8 bit
+    case 3u * 4 + 1: k_gather_scatter<3, 1><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;   // 3 x 8 bit
+    case 2u * 4 + 2: k_gather_scatter<2, 2><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;   // 1 x 16 bit
+    case 6u * 4 + 2: k_gather_scatter<6, 2><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;   // 3 x 16 bit
     default: return cudaErrorInvalidValue;
     }
     return cudaGetLastError();
@@ -410,27 +418,35 @@ cudaError_t launch_mask_popcount(const uint32_t* d_masks, size_t stride_w, uint3
     k_mask_popcount<<<dim3(gx, (unsigned)F), 256, 0, st>>>(d_masks, stride_w, nwords, d_out);
     return cudaGetLastError();
 }
-template <int PB>
+template <int PB, int RS>
 static cudaError_t launch_apply_sweep_t(const ApplyChain& A, int sm_count, cudaStream_t st) {
     int per_sm = 1;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_apply_sweep<PB>, AP_THREADS, 0);
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_apply_sweep<PB, RS>, AP_THREADS, 0);
     if (e != cudaSuccess) return e;
     if (per_sm < 1) per_sm = 1;
     const uint32_t slots = (uint32_t)(sm_count > 0 ? sm_count : 1) * (uint32_t)per_sm;
     const uint32_t rounds = (A.ntiles + slots - 1u) / slots;          // every CTA sweeps the same number of tiles, or one fewer
-    k_apply_sweep<PB><<<(A.ntiles + rounds - 1u) / rounds, AP_THREADS, 0, st>>>(A);
+    k_apply_sweep<PB, RS><<<(A.ntiles + rounds - 1u) / rounds, AP_THREADS, 0, st>>>(A);
     return cudaGetLastError();
 }
 cudaError_t launch_apply_chain(const ApplyChain& A, int sm_count, cudaStream_t st) {
     if (A.count == 0 || A.ntiles == 0) return cudaSuccess;
+    // (pixel bytes, residual sample bytes) as in launch_gather_scatter; 0: no residual pair, the plain sweep
+    const uint32_t key = A.pix_bytes * 4u + (A.residual ? A.sample_bytes : 0u);
+    if (!(key == 1u * 4 || key == 2u * 4 || key == 3u * 4 || key == 6u * 4 || key == 1u * 4 + 1 || key == 3u * 4 + 1 ||
+          key == 2u * 4 + 2 || key == 6u * 4 + 2))
+        return cudaErrorInvalidValue;
     k_tile_count<<<dim3((A.ntiles + 7u) / 8u, A.count), 256, 0, st>>>(A);
     k_tile_scan<<<A.count, 1024, 0, st>>>(A);
-    switch (A.pix_bytes) {
-    case 1: return launch_apply_sweep_t<1>(A, sm_count, st);
-    case 2: return launch_apply_sweep_t<2>(A, sm_count, st);
-    case 3: return launch_apply_sweep_t<3>(A, sm_count, st);
-    case 6: return launch_apply_sweep_t<6>(A, sm_count, st);
-    default: return cudaErrorInvalidValue;
+    switch (key) {
+    case 1u * 4: return launch_apply_sweep_t<1, 0>(A, sm_count, st);
+    case 2u * 4: return launch_apply_sweep_t<2, 0>(A, sm_count, st);
+    case 3u * 4: return launch_apply_sweep_t<3, 0>(A, sm_count, st);
+    case 6u * 4: return launch_apply_sweep_t<6, 0>(A, sm_count, st);
+    case 1u * 4 + 1: return launch_apply_sweep_t<1, 1>(A, sm_count, st);
+    case 3u * 4 + 1: return launch_apply_sweep_t<3, 1>(A, sm_count, st);
+    case 2u * 4 + 2: return launch_apply_sweep_t<2, 2>(A, sm_count, st);
+    default: return launch_apply_sweep_t<6, 2>(A, sm_count, st);
     }
 }
 cudaError_t launch_median5(const void* d_in, uint32_t pix_stride, uint32_t H, uint32_t W, int sample_bytes, void* d_out, cudaStream_t st) {

@@ -39,6 +39,7 @@ struct PairJob {
 struct GatherJob {
     const uint32_t* mask;     // n bits, natural packing
     const uint8_t* frame;     // gather: source (curr) frame; scatter: unused
+    const uint8_t* prev;      // residual gather: the pair's previous frame (values = curr - prev per sample); otherwise unused
     uint8_t* values;          // gather: output; scatter: input (rank-ordered pixel values)
     uint8_t* out_frame;       // scatter: destination frame (already holds the base frame)
     uint32_t npix;
@@ -60,6 +61,8 @@ struct ApplyChain {
     uint32_t npix, ntiles, count, pix_bytes;
     const uint8_t* values;      // rank-ordered pixel values of every pair, back to back
     const uint64_t* value_off;  // [count + 1] byte offsets of each pair's values
+    const uint8_t* residual;    // [count] 1: pair t's values are residuals, added per sample mod 2^(8 sample_bytes); NULL: all plain
+    uint32_t sample_bytes;
     uint32_t* tile_pfx;         // [count][ntiles]: set bits per tile (k_tile_count), then set bits of the earlier tiles (k_tile_scan)
     uint32_t* totals;           // [count] set bits per pair
     uint32_t* first_bad;        // first pair whose value bytes do not match its mask (UINT32_MAX: none); pairs from there are not applied
@@ -101,13 +104,16 @@ cudaError_t launch_witness(const FrameJob* d_jobs, int F, uint32_t max_centuries
 cudaError_t launch_expand(const FrameJob* d_jobs, int F, uint32_t max_centuries, int sm_count, uint32_t* d_scratch, uint32_t* d_consumed,
                           cudaStream_t st);
 uint32_t gather_chunks(uint32_t npix);
+// resid_sample_bytes: 0 gathers the current frame's samples; 1 or 2 gathers curr - prev per sample of that width (gather only,
+// pix_bytes / resid_sample_bytes channels of 1 or 3)
 cudaError_t launch_gather_scatter(const GatherJob* d_jobs, int F, int scatter, uint32_t npix, uint32_t pix_bytes, uint32_t* d_counts,
-                                  uint32_t* d_totals, cudaStream_t st);
+                                  uint32_t* d_totals, cudaStream_t st, uint32_t resid_sample_bytes = 0);
 // decode side of a group (rbf_k4c_apply.cuh): masks of the raw-passthrough jobs (l == 0) from their bitmap slots; set bits per mask
 cudaError_t launch_raw_masks(const FrameJob* d_jobs, int F, uint32_t npix, cudaStream_t st);
 cudaError_t launch_mask_popcount(const uint32_t* d_masks, size_t stride_w, uint32_t npix, int F, uint32_t* d_out, int sm_count,
                                  cudaStream_t st);
-// K4c: tile counts, tile scan (+ the ivc:882 check) and the chained sweep; *A.first_bad must hold UINT32_MAX before the launch
+// K4c: tile counts, tile scan (+ the ivc:882 check) and the chained sweep; *A.first_bad must hold UINT32_MAX before the launch.
+// A.residual == NULL runs the plain sweep, which has no residual branch at all
 cudaError_t launch_apply_chain(const ApplyChain& A, int sm_count, cudaStream_t st);
 cudaError_t launch_median5(const void* d_in, uint32_t pix_stride, uint32_t H, uint32_t W, int sample_bytes, void* d_out, cudaStream_t st);
 cudaError_t launch_bitrev(uint32_t* d_words, size_t nwords, int sm_count, cudaStream_t st);

@@ -343,13 +343,17 @@ class VideoFrameCompressor:
 
 _INTER_TAG_V1 = b"\xff\xff\xff\xffRBF1"   # round-1 layout: raw-passthrough masks stored as plain np.packbits bytes
 _INTER_TAG = b"\xff\xff\xff\xffRBF2"      # current: raw-passthrough masks zlib-compressed (a static scene costs ~1 KB, not n/8 B)
-# neither can be a FixedVideoCompressor payload (height 0xFFFFFFFF).  NOTE: inter payloads exist only in this implementation --
+_INTER_TAG_V3 = b"\xff\xff\xff\xffRBF3"   # value_coding "adaptive": RBF2 plus a vmode byte after the raw flag (0 values, 1 residuals)
+# none can be a FixedVideoCompressor payload (height 0xFFFFFFFF).  NOTE: inter payloads exist only in this implementation --
 # the reference's decoder knows keyframes only (ivc:1124); files written with keyframe_interval=1 are interchangeable.
+_INTER_TAGS = (_INTER_TAG, _INTER_TAG_V1, _INTER_TAG_V3)
 
 
 class _InterPayload:
-    """The fields of one inter-frame payload (ImprovedVideoCompressor._parse_inter); the byte fields are views of the payload."""
-    __slots__ = ("v1", "h", "w", "isz", "ch", "raw", "k", "l", "wlen", "ones", "mask_bytes", "witness_bytes", "vcount", "vz")
+    """The fields of one inter-frame payload (ImprovedVideoCompressor._parse_inter); the byte fields are views of the payload.
+    vmode 1: the value stream holds residuals (curr - prev) mod 2^(8 isz) per sample instead of the current samples."""
+    __slots__ = ("v1", "h", "w", "isz", "ch", "raw", "vmode", "k", "l", "wlen", "ones", "mask_bytes", "witness_bytes", "vcount",
+                 "vz")
 
 
 class _InterJob:
@@ -376,6 +380,11 @@ class ImprovedVideoCompressor:
       "zlib"  (default) zlib level 9 on the CPU: keyframe_interval=1 writes exactly the reference's bytes;
       "gpu"   every zlib stream of the payloads (keyframe blobs, changed values, raw-passthrough masks) is coded on the GPU
               (deflate.py): other compressed bytes, the same decoded data, read by the unchanged decoders.
+    `value_coding`, what an inter frame's value stream holds:
+      "plain"     (default) the current frame's samples at the changed pixels ('RBF2' payloads);
+      "adaptive"  per inter frame, whichever zlib stream is shorter: those samples, or the residuals (curr - prev) mod 2^bits per
+                  sample; a tie goes to the samples ('RBF3' payloads, whose vmode byte says which).  The decoder adds residuals to
+                  the previous frame, which equals the encoder's original previous frame in both inter_frame_modes.
     """
 
     def __init__(self, noise_tolerance: float = 10.0, keyframe_interval: int = 30, min_diff_threshold: float = 3.0,
@@ -394,6 +403,7 @@ class ImprovedVideoCompressor:
         self.inter_frame_mode = "lossless"
         self.inter_frame_threshold = 0.0
         self.entropy_coder = "zlib"
+        self.value_coding = "plain"
         _cabi.ctx()                                                                 # fail now if there is no H100
 
     # ------------------------------------------------------------------ encode
@@ -404,16 +414,29 @@ class ImprovedVideoCompressor:
         return np.packbits(np.unpackbits(mask_row, bitorder="little")[:n]).tobytes()
 
     @staticmethod
-    def _inter_payload(shape, itemsize, ch, r, bm_row, wt_row, mask_row, values) -> bytes:
-        """Assemble one inter-frame payload (runs in a worker thread; the zlib calls release the GIL)."""
-        vz = zlib.compress(values.tobytes(), 9)
-        rz = zlib.compress(ImprovedVideoCompressor._raw_mask_bits(shape, mask_row), 9) if r.raw else None
-        return ImprovedVideoCompressor._inter_layout(shape, itemsize, ch, r, bm_row, wt_row, rz, vz, values.size)
+    def _choose_values(vz: bytes, dz: Optional[bytes]):
+        """-> (value stream, vmode): the residual stream `dz` when it is strictly shorter than the values' `vz`, else `vz`; vmode is
+        None (an 'RBF2' payload) when there is no residual stream."""
+        if dz is None:
+            return vz, None
+        return (dz, 1) if len(dz) < len(vz) else (vz, 0)
 
     @staticmethod
-    def _inter_layout(shape, itemsize, ch, r, bm_row, wt_row, rz, vz, vcount) -> bytes:
-        """The inter-frame byte layout around the compressed raw mask `rz` (raw pairs only) and changed values `vz`."""
-        hdr = _INTER_TAG + struct.pack("<IIIBB", shape[0], shape[1], itemsize, ch, 1 if r.raw else 0)
+    def _inter_payload(shape, itemsize, ch, r, bm_row, wt_row, mask_row, values, resids=None) -> bytes:
+        """Assemble one inter-frame payload (runs in a worker thread; the zlib calls release the GIL).  With `resids` (adaptive
+        value coding) both value streams are compressed and the shorter one is kept."""
+        vz, vmode = ImprovedVideoCompressor._choose_values(zlib.compress(values.tobytes(), 9),
+                                                           None if resids is None else zlib.compress(resids.tobytes(), 9))
+        rz = zlib.compress(ImprovedVideoCompressor._raw_mask_bits(shape, mask_row), 9) if r.raw else None
+        return ImprovedVideoCompressor._inter_layout(shape, itemsize, ch, r, bm_row, wt_row, rz, vz, values.size, vmode)
+
+    @staticmethod
+    def _inter_layout(shape, itemsize, ch, r, bm_row, wt_row, rz, vz, vcount, vmode=None) -> bytes:
+        """The inter-frame byte layout around the compressed raw mask `rz` (raw pairs only) and changed values `vz`.  vmode None
+        writes 'RBF2'; 0 (values) or 1 (residuals) writes 'RBF3', which carries it in one byte after the raw flag."""
+        hdr = (_INTER_TAG if vmode is None else _INTER_TAG_V3) + struct.pack("<IIIBB", shape[0], shape[1], itemsize, ch, 1 if r.raw else 0)
+        if vmode is not None:
+            hdr += struct.pack("<B", vmode)
         body = struct.pack("<dIIQ", r.k, r.l, r.wlen, r.ones)
         if r.raw:
             body += struct.pack("<I", len(rz)) + rz + struct.pack("<I", 0)
@@ -428,11 +451,18 @@ class ImprovedVideoCompressor:
         """The fields of an inter-frame payload (the inverse of _inter_layout; also reads round 1's 'RBF1' tag, whose raw masks are
         plain np.packbits bytes).  Nothing is decompressed: `mask_bytes` is the stored raw mask or bitmap, `vz` the value stream."""
         p = _InterPayload()
-        p.v1 = payload[:len(_INTER_TAG_V1)] == _INTER_TAG_V1
+        tag = bytes(payload[:len(_INTER_TAG)])
+        p.v1 = tag == _INTER_TAG_V1
         mv = memoryview(payload)
         pos = len(_INTER_TAG)
         p.h, p.w, p.isz, p.ch, p.raw = struct.unpack_from("<IIIBB", payload, pos)
         pos += struct.calcsize("<IIIBB")
+        p.vmode = 0
+        if tag == _INTER_TAG_V3:
+            (p.vmode,) = struct.unpack_from("<B", payload, pos)
+            pos += 1
+            if p.vmode not in (0, 1):
+                raise ValueError(f"corrupt inter frame: value coding {p.vmode} is neither 0 (values) nor 1 (residuals)")
         p.k, p.l, p.wlen, p.ones = struct.unpack_from("<dIIQ", payload, pos)
         pos += struct.calcsize("<dIIQ")
         (bl,) = struct.unpack_from("<I", payload, pos); pos += 4
@@ -466,20 +496,33 @@ class ImprovedVideoCompressor:
                     self._gpu_inter_payloads(st, shape, dtype.itemsize, ch, idxs, res, bms, wts, masks, out, pool)
                     continue
                 gathered = st.gather_changed(len(idxs))            # N1: changed values of every pair, one launch, one copy
+                resids = self._with_residuals(st, st.gather_changed, len(idxs)) if self.value_coding == "adaptive" else None
                 for j, i in enumerate(idxs):
                     r = res[j]
                     if r.resid and self.inter_frame_mode != "lossless":
                         out[i] = None                              # not exactly representable: keyframe instead
                         continue
                     out[i] = pool.submit(self._inter_payload, shape, dtype.itemsize, ch, r, bms[j], wts[j],
-                                         masks[j] if (masks is not None and r.raw) else None, gathered[j])
+                                         masks[j] if (masks is not None and r.raw) else None, gathered[j],
+                                         None if resids is None else resids[j])
         finally:
             st.close()
         return out
 
+    @staticmethod
+    def _with_residuals(st: FrameStream, fn, pairs: int):
+        """fn(pairs) with the stream's gathers returning residuals (value_mode 1) instead of the current samples."""
+        st.set_option("value_mode", 1)
+        try:
+            return fn(pairs)
+        finally:
+            st.set_option("value_mode", 0)
+
     def _gpu_inter_payloads(self, st, shape, itemsize, ch, idxs, res, bms, wts, masks, out, pool) -> None:
-        """entropy_coder "gpu": changed values deflated where they were gathered (N1 + N4), raw masks in one batch."""
+        """entropy_coder "gpu": changed values (and, adaptive, their residuals) deflated where they were gathered (N1 + N4), raw masks
+        in one batch."""
         vzs = st.zlib_changed(len(idxs))
+        dzs = self._with_residuals(st, st.zlib_changed, len(idxs)) if self.value_coding == "adaptive" else [None] * len(idxs)
         voffs = st.changed_offsets(len(idxs))
         keep = [j for j, i in enumerate(idxs) if not (res[j].resid and self.inter_frame_mode != "lossless")]
         raw_js = [j for j in keep if res[j].raw]
@@ -489,7 +532,8 @@ class ImprovedVideoCompressor:
                 out[i] = None                                      # not exactly representable: keyframe instead
                 continue
             vcount = int(voffs[j + 1] - voffs[j]) // itemsize
-            out[i] = pool.submit(self._inter_layout, shape, itemsize, ch, res[j], bms[j], wts[j], rzs.get(j), vzs[j], vcount)
+            vz, vmode = self._choose_values(vzs[j], dzs[j])
+            out[i] = pool.submit(self._inter_layout, shape, itemsize, ch, res[j], bms[j], wts[j], rzs.get(j), vz, vcount, vmode)
 
     def _keyframe_job(self, frame, pool):
         """Callable returning the keyframe payload of `frame`: zlib level 9 in the pool, or coded on the GPU now."""
@@ -501,6 +545,8 @@ class ImprovedVideoCompressor:
     def compress_video(self, frames: List[np.ndarray], output_path: str = None, input_color_space: str = "BGR") -> Dict:
         if self.entropy_coder not in ("zlib", "gpu"):
             raise ValueError(f"entropy_coder must be 'zlib' or 'gpu', not {self.entropy_coder!r}")
+        if self.value_coding not in ("plain", "adaptive"):
+            raise ValueError(f"value_coding must be 'plain' or 'adaptive', not {self.value_coding!r}")
         if not frames:
             raise ValueError("No frames provided for compression")                 # ivc:372-373
         start_time = time.time()
@@ -620,7 +666,7 @@ class ImprovedVideoCompressor:
                 raise IndexError("list index out of range")
             if ones[i] != j.p.ones:                          # the reference would silently return the base frame (ivc:882)
                 raise ValueError(f"corrupt inter frame: the decoded mask selects {int(ones[i])} pixels, the payload announces {j.p.ones}")
-        applied = st.apply_chain(base, [j.values_arr for j in group])
+        applied = st.apply_chain(base, [j.values_arr for j in group], residual=[j.p.vmode for j in group])
         if not np.array_equal(applied, ones):
             raise ValueError(f"corrupt inter frame: {applied.tolist()} pixels applied, {ones.tolist()} expected")
         return st.download_batch((base + 1) % st.max_frames, m)
@@ -677,7 +723,7 @@ class ImprovedVideoCompressor:
         streams: Dict[tuple, FrameStream] = {}
         pool = ThreadPoolExecutor(self.num_threads)
         try:
-            jobs = [self._start_inter(c, pool) if c[:len(_INTER_TAG)] in (_INTER_TAG, _INTER_TAG_V1)
+            jobs = [self._start_inter(c, pool) if c[:len(_INTER_TAG)] in _INTER_TAGS
                     else pool.submit(self.compressor.decompress_frame, c) for c in compressed_frames]
             i = 0
             while i < len(jobs):

@@ -47,7 +47,8 @@ class FrameStream:
             self.set_option(key, val)
 
     def set_option(self, key: str, value: int) -> None:
-        """Per-stream option of the C ABI (rbf_stream_set_option): k1_only, mask_mode, gray_mode."""
+        """Per-stream option of the C ABI (rbf_stream_set_option): k1_only, mask_mode, gray_mode, value_mode (0: gather_changed and
+        zlib_changed return the current samples; 1: residuals (curr - prev) mod 2^bits per sample)."""
         _cabi.check(_cabi.lib().rbf_stream_set_option(self._h, key.encode(), int(value)), _cabi.ctx())
         if key == "k1_only":
             self.k1_only = bool(value)
@@ -201,17 +202,24 @@ class FrameStream:
         self.pairs = 0
         return consumed, ones
 
-    def apply_chain(self, base_frame: int, values: Sequence[np.ndarray]) -> np.ndarray:
+    def apply_chain(self, base_frame: int, values: Sequence[np.ndarray], residual: Optional[Sequence[int]] = None) -> np.ndarray:
         """Frame base_frame+1+i = frame base_frame+i with mask slot i applied, values[i] replacing its set pixels in rank order
-        (ivc:849-909), for i < len(values); slots are taken modulo max_frames.  -> uint64[count] pixels applied per pair: 0 from
-        the first pair whose value count does not match its mask (ivc:882), whose frame and every later one are not written."""
+        (ivc:849-909), for i < len(values); slots are taken modulo max_frames.  residual[i] = 1 adds values[i] to the set pixels
+        per sample (mod 2^bits) instead: the residuals a value_mode=1 gather returns.  -> uint64[count] pixels applied per pair: 0
+        from the first pair whose value count does not match its mask (ivc:882), whose frame and every later one are not written."""
         parts = [memoryview(np.ascontiguousarray(v)).cast("B") for v in values]
         offs = np.zeros(len(parts) + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([p.nbytes for p in parts])
         buf = np.frombuffer(b"".join(parts), dtype=np.uint8)
         applied = np.zeros(len(parts), dtype=np.uint64)
-        _cabi.check(_cabi.lib().rbf_stream_apply_chain(self._h, int(base_frame), len(parts), _cabi.ptr(buf) if buf.size else None,
-                                                       _cabi.ptr(offs), _cabi.ptr(applied)), _cabi.ctx())
+        flags = None
+        if residual is not None:
+            flags = np.ascontiguousarray(np.asarray(residual, dtype=np.uint8))
+            if flags.shape != (len(parts),):
+                raise ValueError("one residual flag per pair")
+        _cabi.check(_cabi.lib().rbf_stream_apply_chain_modes(self._h, int(base_frame), len(parts), _cabi.ptr(buf) if buf.size else None,
+                                                             _cabi.ptr(offs), _cabi.ptr(flags) if flags is not None else None,
+                                                             _cabi.ptr(applied)), _cabi.ctx())
         return applied
 
     def download_batch(self, first: int, count: int) -> np.ndarray:
