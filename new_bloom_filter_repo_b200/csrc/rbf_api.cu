@@ -41,24 +41,14 @@ struct rbf_ctx {
     cudaEvent_t ev_fork = nullptr, ev_wit = nullptr, ev_k1[8] = {nullptr}, ev_d2h = nullptr;
     int encode_ranges = 1;            // rbf_stream_encode: K1/K2 pipelined over this many ranges of pairs (1 = serial, the default; a K2 CTA
                                       // takes a whole SM's shared memory, so K1 and K2 overlap on different SMs)
-    int k1_ctas_per_sm = 32;          // grid cap of K1 (pipelined encodes use pipe_k1_ctas_per_sm so that K2 finds room beside it)
-    int pipe_k1_ctas_per_sm = 4;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaDeviceProp prop;
-    int sm_count = 0;
-    int k1_variant = 0;
-    int insert_variant = 1; // 1: dense warp-compacted K2 building the arrays in shared memory (default); 0: per-lane K2, RED.OR into L2
-    int query_variant = 5;  // 0: per-lane; 1: staged A->B->C rings, L2 tail; 2, 3, 4: as 5; 5: decade tiles with carried stage-B
-                            // batches (half tiles for 2^23 < m <= 2^24, ring kernel beyond); 6: half-decade tiles for every m <= 2^24
+    LaunchCfg L;            // launcher options and the kernel counter
     int k1_only = 0;        // stop after K1 (mask + counts): VideoFrameCompressor._calculate_frame_diff
     int mask_mode = 0;      // 0: |dY| > thr (ivc:808); 1: additionally any byte of the pixel differs
-    int query_smem_cap = 0;
-    int query_warps = 0;    // warps per CTA of the tile query kernel (0 = its compiled maximum, 28)
     int kq_ranges = 1;      // > 1: K2 of range r+1 runs beside K3 of range r (see stream_encode_pipelined)
-    int k2_clusters[9] = {0};   // resident K2 clusters of 1..8 CTAs, measured by the first K2 launch of each shape.  Not at
-                                // creation: querying it there slowed 8K K3 (which never uses this kernel) by 12 %, cause unknown
     char err[512];
-    int64_t launches = 0, h2d = 0, d2h = 0;
+    int64_t h2d = 0, d2h = 0;
     std::vector<void*> scratch;
     std::vector<size_t> scratch_sz;
     // NCCL (dlopen'ed)
@@ -84,13 +74,21 @@ static int set_err(rbf_ctx* c, int code, const char* fmt, ...) {
             return set_err(ctx, e__ == cudaErrorMemoryAllocation ? RBF_ERR_OOM : RBF_ERR_CUDA, "%s:%d %s: %s", \
                            __FILE__, __LINE__, #call, cudaGetErrorString(e__));                               \
     } while (0)
-#define LAUNCH(ctx, call)  \
-    do {                   \
-        CK(ctx, call);     \
-        (ctx)->launches++; \
-    } while (0)
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// Scratch slots of a context (scratch_get).  Entry points that name the same slot overwrite each other's contents: nothing in a
+// slot outlives the call that wrote it.
+enum ScratchSlot {
+    kScrBytes, kScrResult, kScrOffsets,           // byte per item / bit, check results, string offsets (filters, single-mask coder)
+    kScrMask, kScrBits, kScrPass, kScrWit,        // the single-mask coder's FrameJob buffers
+    kScrSmall,                                    // its counts, prefix and job; decode_verify's mismatch counts
+    kScrValues,                                   // changed values: gather_changed, zlib_changed, apply_diff, apply_chain
+    kScrGatherJobs, kScrApplyMask, kScrMedianIn, kScrMedianOut,
+    kScrGatherCounts,                             // per-chunk set-bit counts of the gather / scatter kernels
+    kScrZlibRes, kScrZlibOut, kScrZlibStage, kScrZlibSegs, kScrZlibCopies, kScrZlibSmall, kScrZlibIn,
+    kScrDecodeCounts, kScrChainSmall, kScrChainTiles,   // decode_masks' counts; apply_chain's offsets + flags + totals, tile prefix
+};
 
 static int scratch_get(rbf_ctx* c, int slot, size_t bytes, void** out) {
     if ((int)c->scratch.size() <= slot) { c->scratch.resize(slot + 1, nullptr); c->scratch_sz.resize(slot + 1, 0); }
@@ -217,8 +215,8 @@ extern "C" int rbf_ctx_create(int device, rbf_ctx** out) {
         delete c;
         return set_err(nullptr, RBF_ERR_NO_DEVICE, "device is sm_%d%d; this library is built for sm_90a only", maj, mn);
     }
-    c->sm_count = c->prop.multiProcessorCount;
-    c->query_smem_cap = query_max_smem_bytes();
+    c->L.sm_count = c->prop.multiProcessorCount;
+    c->L.query_smem_cap = query_max_smem_bytes();
     if ((e = cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking)) != cudaSuccess ||
         (e = cudaEventCreate(&c->ev0)) != cudaSuccess || (e = cudaEventCreate(&c->ev1)) != cudaSuccess) {
         delete c;
@@ -256,7 +254,7 @@ extern "C" int rbf_device_info(rbf_ctx* c, char* name, int name_len, int* sm_cou
                                uint64_t* total_mem) {
     if (!c) return set_err(nullptr, RBF_ERR_INVALID, "ctx is NULL");
     if (name && name_len > 0) snprintf(name, name_len, "%s", c->prop.name);
-    if (sm_count) *sm_count = c->sm_count;
+    if (sm_count) *sm_count = c->L.sm_count;
     if (cc_major) *cc_major = c->prop.major;
     if (cc_minor) *cc_minor = c->prop.minor;
     if (total_mem) *total_mem = c->prop.totalGlobalMem;
@@ -264,31 +262,31 @@ extern "C" int rbf_device_info(rbf_ctx* c, char* name, int name_len, int* sm_cou
 }
 extern "C" int rbf_set_option(rbf_ctx* c, const char* key, int64_t v) {
     if (!c || !key) return set_err(c, RBF_ERR_INVALID, "rbf_set_option: NULL");
-    if (!strcmp(key, "k1_variant")) { c->k1_variant = (int)v; return RBF_OK; }
-    if (!strcmp(key, "query_variant")) { c->query_variant = (int)(v < 0 ? 0 : (v > 6 ? 6 : v)); return RBF_OK; }
-    if (!strcmp(key, "insert_variant")) { c->insert_variant = v ? 1 : 0; return RBF_OK; }
+    if (!strcmp(key, "k1_variant")) { c->L.k1_variant = (int)v; return RBF_OK; }
+    if (!strcmp(key, "query_variant")) { c->L.query_variant = (int)(v < 0 ? 0 : (v > 6 ? 6 : v)); return RBF_OK; }
+    if (!strcmp(key, "insert_variant")) { c->L.insert_variant = v ? 1 : 0; return RBF_OK; }
     if (!strcmp(key, "host_chunk_frames")) { c->host_chunk_frames = (int)v; return RBF_OK; }
     if (!strcmp(key, "k1_only")) { c->k1_only = v ? 1 : 0; return RBF_OK; }        // default of streams created afterwards
     if (!strcmp(key, "mask_mode")) { c->mask_mode = v ? 1 : 0; return RBF_OK; }    // (per-stream: rbf_stream_set_option)
-    if (!strcmp(key, "query_warps")) { c->query_warps = (int)v; return RBF_OK; }
+    if (!strcmp(key, "query_warps")) { c->L.query_warps = (int)v; return RBF_OK; }
     if (!strcmp(key, "kq_ranges")) { c->kq_ranges = (int)(v < 1 ? 1 : (v > 8 ? 8 : v)); return RBF_OK; }
     if (!strcmp(key, "encode_ranges")) { c->encode_ranges = (int)(v < 1 ? 1 : (v > 8 ? 8 : v)); return RBF_OK; }
-    if (!strcmp(key, "k1_ctas_per_sm")) { c->k1_ctas_per_sm = (int)(v < 1 ? 1 : (v > 64 ? 64 : v)); return RBF_OK; }
-    if (!strcmp(key, "pipe_k1_ctas_per_sm")) { c->pipe_k1_ctas_per_sm = (int)(v < 1 ? 1 : (v > 64 ? 64 : v)); return RBF_OK; }
+    if (!strcmp(key, "k1_ctas_per_sm")) { c->L.k1_ctas_per_sm = (int)(v < 1 ? 1 : (v > 64 ? 64 : v)); return RBF_OK; }
+    if (!strcmp(key, "pipe_k1_ctas_per_sm")) { c->L.pipe_k1_ctas_per_sm = (int)(v < 1 ? 1 : (v > 64 ? 64 : v)); return RBF_OK; }
     if (!strcmp(key, "query_smem_bytes")) {
-        c->query_smem_cap = (int)((v <= 0 || v > query_max_smem_bytes()) ? query_max_smem_bytes() : v);
+        c->L.query_smem_cap = (int)((v <= 0 || v > query_max_smem_bytes()) ? query_max_smem_bytes() : v);
         return RBF_OK;
     }
     return set_err(c, RBF_ERR_INVALID, "unknown option %s", key);
 }
 extern "C" int64_t rbf_get_counter(rbf_ctx* c, const char* key) {
     if (!c || !key) return -1;
-    if (!strcmp(key, "kernel_launches")) return c->launches;
+    if (!strcmp(key, "kernel_launches")) return c->L.launches;
     if (!strcmp(key, "h2d_bytes")) return c->h2d;
     if (!strcmp(key, "d2h_bytes")) return c->d2h;
     return -1;
 }
-extern "C" int rbf_reset_counters(rbf_ctx* c) { if (!c) return RBF_ERR_INVALID; c->launches = c->h2d = c->d2h = 0; return RBF_OK; }
+extern "C" int rbf_reset_counters(rbf_ctx* c) { if (!c) return RBF_ERR_INVALID; c->L.launches = c->h2d = c->d2h = 0; return RBF_OK; }
 // before the bit arrays are overwritten: the slot packing of a pending all-gather must have read them
 static int wait_pack(rbf_ctx* c) {
     if (c->pack_pending) { CK(c, cudaStreamWaitEvent(c->st, c->ev_pack, 0)); c->pack_pending = false; }
@@ -299,7 +297,7 @@ static const long long kPeerTimeoutCycles = 6000000000LL;    // ~3 s of SM clock
 static int join_comm(rbf_ctx* c) {
     if (c->comm_pending) { CK(c, cudaStreamWaitEvent(c->st, c->ev_comm, 0)); c->comm_pending = false; c->pack_pending = false; }
     if (c->peer_wait_pending) {                                // the other ranks' slots of the last exchange
-        LAUNCH(c, launch_peer_wait(c->peer_flags[c->peer_rank], c->peer_nranks, c->peer_seq, kPeerTimeoutCycles, c->peer_err, c->st));
+        CK(c, launch_peer_wait(c->L, c->peer_flags[c->peer_rank], c->peer_nranks, c->peer_seq, kPeerTimeoutCycles, c->peer_err, c->st));
         c->peer_wait_pending = false;
     }
     return RBF_OK;
@@ -388,10 +386,10 @@ static int filter_items_u32(rbf_filter* f, const uint32_t* items, uint32_t count
     if (count == 0) return RBF_OK;
     void *d_items, *d_res;
     int rc;
-    if ((rc = scratch_get(c, 0, (size_t)count * 4, &d_items))) return rc;
-    if ((rc = scratch_get(c, 1, (size_t)count, &d_res))) return rc;
+    if ((rc = scratch_get(c, kScrBytes, (size_t)count * 4, &d_items))) return rc;
+    if ((rc = scratch_get(c, kScrResult, (size_t)count, &d_res))) return rc;
     CK(c, cudaMemcpyAsync(d_items, items, (size_t)count * 4, cudaMemcpyHostToDevice, c->st)); c->h2d += (size_t)count * 4;
-    LAUNCH(c, launch_items_u32(f->d_job, (const uint32_t*)d_items, count, (uint8_t*)d_res, insert, c->sm_count, c->st));
+    CK(c, launch_items_u32(c->L, f->d_job, (const uint32_t*)d_items, count, (uint8_t*)d_res, insert, c->st));
     if (!insert) { CK(c, cudaMemcpyAsync(out, d_res, count, cudaMemcpyDeviceToHost, c->st)); c->d2h += count; }
     CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
@@ -411,14 +409,14 @@ static int filter_items_str(rbf_filter* f, const uint8_t* blob, const uint64_t* 
     const size_t blob_bytes = (size_t)offs[count];
     void *d_blob, *d_offs, *d_res;
     int rc;
-    if ((rc = scratch_get(c, 0, blob_bytes + 16, &d_blob))) return rc;
-    if ((rc = scratch_get(c, 1, (size_t)count, &d_res))) return rc;
-    if ((rc = scratch_get(c, 2, ((size_t)count + 1) * 8, &d_offs))) return rc;
+    if ((rc = scratch_get(c, kScrBytes, blob_bytes + 16, &d_blob))) return rc;
+    if ((rc = scratch_get(c, kScrResult, (size_t)count, &d_res))) return rc;
+    if ((rc = scratch_get(c, kScrOffsets, ((size_t)count + 1) * 8, &d_offs))) return rc;
     if (blob_bytes) { CK(c, cudaMemcpyAsync(d_blob, blob, blob_bytes, cudaMemcpyHostToDevice, c->st)); }
     CK(c, cudaMemcpyAsync(d_offs, offs, ((size_t)count + 1) * 8, cudaMemcpyHostToDevice, c->st));
     c->h2d += blob_bytes + ((size_t)count + 1) * 8;
-    LAUNCH(c, launch_items_str(f->d_job, (const uint8_t*)d_blob, (const uint64_t*)d_offs, count, (uint8_t*)d_res, insert,
-                               standard_k, c->sm_count, c->st));
+    CK(c, launch_items_str(c->L, f->d_job, (const uint8_t*)d_blob, (const uint64_t*)d_offs, count, (uint8_t*)d_res, insert,
+                               standard_k, c->st));
     if (!insert) { CK(c, cudaMemcpyAsync(out, d_res, count, cudaMemcpyDeviceToHost, c->st)); c->d2h += count; }
     CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
@@ -436,8 +434,8 @@ extern "C" int rbf_filter_get_bits(rbf_filter* f, uint8_t* out) {
     if (!f || !out) return set_err(f ? f->c : nullptr, RBF_ERR_INVALID, "rbf_filter_get_bits: NULL");
     rbf_ctx* c = f->c;
     void* d_bytes; int rc;
-    if ((rc = scratch_get(c, 0, f->size, &d_bytes))) return rc;
-    LAUNCH(c, launch_unpack_bits(f->d_bits, (uint8_t*)d_bytes, f->size, c->sm_count, c->st));
+    if ((rc = scratch_get(c, kScrBytes, f->size, &d_bytes))) return rc;
+    CK(c, launch_unpack_bits(c->L, f->d_bits, (uint8_t*)d_bytes, f->size, c->st));
     CK(c, cudaMemcpyAsync(out, d_bytes, f->size, cudaMemcpyDeviceToHost, c->st)); c->d2h += f->size;
     CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
@@ -446,10 +444,10 @@ extern "C" int rbf_filter_set_bits(rbf_filter* f, const uint8_t* in) {
     if (!f || !in) return set_err(f ? f->c : nullptr, RBF_ERR_INVALID, "rbf_filter_set_bits: NULL");
     rbf_ctx* c = f->c;
     void* d_bytes; int rc;
-    if ((rc = scratch_get(c, 0, f->size, &d_bytes))) return rc;
+    if ((rc = scratch_get(c, kScrBytes, f->size, &d_bytes))) return rc;
     CK(c, cudaMemcpyAsync(d_bytes, in, f->size, cudaMemcpyHostToDevice, c->st)); c->h2d += f->size;
     CK(c, cudaMemsetAsync(f->d_bits, 0, f->words * 4, c->st));
-    LAUNCH(c, launch_pack_bytes((const uint8_t*)d_bytes, f->d_bits, f->size, c->sm_count, c->st));
+    CK(c, launch_pack_bytes(c->L, (const uint8_t*)d_bytes, f->d_bits, f->size, c->st));
     CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
 }
@@ -461,6 +459,28 @@ extern "C" int rbf_filter_set_bits(rbf_filter* f, const uint8_t* in) {
 static size_t bit_words_padded(uint64_t nbits) { return align_up((nbits + 31) / 32 + 8, 32); }   // >= 32 B of padding, 128 B multiple
 static size_t pass_words(uint64_t n) { return align_up(((n + 99) / 100) * 4, 32); }
 
+// A FrameJob of n positions over the given bit array, witness and pass mask, with the filter of (l, k*) when l > 0 (l == 0: raw
+// passthrough).  The caller adds the mask it encodes (mask) or decodes into (out_mask, wlen_in).
+static FrameJob frame_job(uint64_t n, uint64_t l, double k_star, const rbf_seeds& sd, uint32_t* bits, uint32_t* witness, uint32_t* pass) {
+    FrameJob J;
+    memset(&J, 0, sizeof J);
+    J.n = (uint32_t)n;
+    if (l) job_set_filter(J, l, k_star, sd);
+    J.bits = bits; J.witness = witness; J.pass = pass;
+    return J;
+}
+
+// Decode (K3 + K4b) of F jobs on the context's stream: the jobs and their century prefix (F + 1 entries) go to the device, every
+// coded job's mask lands in its out_mask and its consumed witness bits in d_consumed.  d_scratch: F * 32 words.
+static int decode_enqueue(rbf_ctx* c, const FrameJob* h_jobs, FrameJob* d_jobs, const uint32_t* h_prefix, uint32_t* d_prefix, int F,
+                          uint32_t max_l, uint32_t ncent, uint32_t* d_scratch, uint32_t* d_consumed) {
+    CK(c, cudaMemcpyAsync(d_jobs, h_jobs, sizeof(FrameJob) * F, cudaMemcpyHostToDevice, c->st));
+    CK(c, cudaMemcpyAsync(d_prefix, h_prefix, 4 * ((size_t)F + 1), cudaMemcpyHostToDevice, c->st));
+    CK(c, launch_query(c->L, d_jobs, d_prefix, F, h_prefix[F], max_l, c->st));
+    CK(c, launch_expand(c->L, d_jobs, F, ncent, d_scratch, d_consumed, c->st));
+    return RBF_OK;
+}
+
 extern "C" int rbf_compress_mask(rbf_ctx* c, const uint8_t* mask, uint64_t n, const rbf_seeds* sd, double k_override,
                                  uint64_t l_override, rbf_mask_info* info, uint8_t* bitmap_out, uint8_t* witness_out) {
     if (!c || !mask || !sd || !info) return set_err(c, RBF_ERR_INVALID, "rbf_compress_mask: NULL argument");
@@ -471,9 +491,9 @@ extern "C" int rbf_compress_mask(rbf_ctx* c, const uint8_t* mask, uint64_t n, co
     const size_t mw = bit_words_padded(n), pw = pass_words(n);
     void *d_bytes, *d_mask, *d_bits, *d_pass, *d_wit, *d_small;
     int rc;
-    if ((rc = scratch_get(c, 0, n, &d_bytes)) || (rc = scratch_get(c, 3, mw * 4, &d_mask)) ||
-        (rc = scratch_get(c, 4, mw * 4, &d_bits)) || (rc = scratch_get(c, 5, pw * 4, &d_pass)) ||
-        (rc = scratch_get(c, 6, mw * 4, &d_wit)) || (rc = scratch_get(c, 7, 4096, &d_small)))
+    if ((rc = scratch_get(c, kScrBytes, n, &d_bytes)) || (rc = scratch_get(c, kScrMask, mw * 4, &d_mask)) ||
+        (rc = scratch_get(c, kScrBits, mw * 4, &d_bits)) || (rc = scratch_get(c, kScrPass, pw * 4, &d_pass)) ||
+        (rc = scratch_get(c, kScrWit, mw * 4, &d_wit)) || (rc = scratch_get(c, kScrSmall, 4096, &d_small)))
         return rc;
     uint32_t* d_cnt = (uint32_t*)d_small;                         // [0] ones, [1] wlen
     uint32_t* d_prefix = d_cnt + 4;                               // [2] cent_prefix
@@ -481,8 +501,8 @@ extern "C" int rbf_compress_mask(rbf_ctx* c, const uint8_t* mask, uint64_t n, co
     CK(c, cudaMemcpyAsync(d_bytes, mask, n, cudaMemcpyHostToDevice, c->st)); c->h2d += n;
     CK(c, cudaMemsetAsync(d_mask, 0, mw * 4, c->st));
     CK(c, cudaMemsetAsync(d_cnt, 0, 16, c->st));
-    LAUNCH(c, launch_pack_bytes((const uint8_t*)d_bytes, (uint32_t*)d_mask, n, c->sm_count, c->st));
-    LAUNCH(c, launch_popcount((const uint32_t*)d_mask, (n + 31) / 32, d_cnt, c->sm_count, c->st));
+    CK(c, launch_pack_bytes(c->L, (const uint8_t*)d_bytes, (uint32_t*)d_mask, n, c->st));
+    CK(c, launch_popcount(c->L, (const uint32_t*)d_mask, (n + 31) / 32, d_cnt, c->st));
     uint32_t h_cnt[4] = {0, 0, 0, 0};
     CK(c, cudaMemcpyAsync(h_cnt, d_cnt, 16, cudaMemcpyDeviceToHost, c->st)); c->d2h += 16;
     CK(c, cudaStreamSynchronize(c->st));
@@ -493,10 +513,8 @@ extern "C" int rbf_compress_mask(rbf_ctx* c, const uint8_t* mask, uint64_t n, co
     if (k_override > 0.0 && !(p >= kPStar)) { k = k_override; l = l_override; coded = !(l == 0 || l >= n); }
     if (!coded) { info->raw = 1; return RBF_OK; }
     info->k = k; info->l = l;
-    FrameJob J; memset(&J, 0, sizeof J);
-    J.n = (uint32_t)n;
-    job_set_filter(J, l, k, *sd);
-    J.mask = (const uint32_t*)d_mask; J.bits = (uint32_t*)d_bits; J.pass = (uint32_t*)d_pass; J.witness = (uint32_t*)d_wit;
+    FrameJob J = frame_job(n, l, k, *sd, (uint32_t*)d_bits, (uint32_t*)d_wit, (uint32_t*)d_pass);
+    J.mask = (const uint32_t*)d_mask;
     info->floor_k = J.floor_k; info->act_T = J.act_T;
     const uint32_t ncent = (uint32_t)((n + 99) / 100);
     uint32_t h_prefix[2] = {0, ncent};
@@ -504,20 +522,20 @@ extern "C" int rbf_compress_mask(rbf_ctx* c, const uint8_t* mask, uint64_t n, co
     CK(c, cudaMemcpyAsync(d_prefix, h_prefix, 8, cudaMemcpyHostToDevice, c->st));
     CK(c, cudaMemsetAsync(d_bits, 0, bit_words_padded(l) * 4, c->st));
     CK(c, cudaMemsetAsync(d_wit, 0, mw * 4, c->st));
-    LAUNCH(c, launch_insert(d_job, 1, ncent, (uint32_t)l, c->insert_variant, c->sm_count, c->k2_clusters, c->st));
-    LAUNCH(c, launch_query(d_job, d_prefix, 1, ncent, (uint32_t)l, c->query_variant, c->sm_count, c->query_smem_cap, c->query_warps, c->st));
-    LAUNCH(c, launch_witness(d_job, 1, ncent, c->sm_count, (uint32_t*)((uint8_t*)d_small + 1024), d_cnt + 1, c->st)); c->launches += 2;
+    CK(c, launch_insert(c->L, d_job, 1, ncent, (uint32_t)l, c->st));
+    CK(c, launch_query(c->L, d_job, d_prefix, 1, ncent, (uint32_t)l, c->st));
+    CK(c, launch_witness(c->L, d_job, 1, ncent, (uint32_t*)((uint8_t*)d_small + 1024), d_cnt + 1, c->st));
     CK(c, cudaMemcpyAsync(h_cnt, d_cnt, 16, cudaMemcpyDeviceToHost, c->st)); c->d2h += 16;
     CK(c, cudaStreamSynchronize(c->st));
     info->wlen = h_cnt[1];
     // after K3b both streams are in packbits order; hand them back unpacked (ivc:266 returns bit_array, witness)
     if (bitmap_out) {
-        LAUNCH(c, launch_unpack_bits_msb((const uint32_t*)d_bits, (uint8_t*)d_bytes, l, c->sm_count, c->st));
+        CK(c, launch_unpack_bits_msb(c->L, (const uint32_t*)d_bits, (uint8_t*)d_bytes, l, c->st));
         CK(c, cudaMemcpyAsync(bitmap_out, d_bytes, l, cudaMemcpyDeviceToHost, c->st)); c->d2h += l;
         CK(c, cudaStreamSynchronize(c->st));
     }
     if (witness_out && info->wlen) {
-        LAUNCH(c, launch_unpack_bits_msb((const uint32_t*)d_wit, (uint8_t*)d_bytes, info->wlen, c->sm_count, c->st));
+        CK(c, launch_unpack_bits_msb(c->L, (const uint32_t*)d_wit, (uint8_t*)d_bytes, info->wlen, c->st));
         CK(c, cudaMemcpyAsync(witness_out, d_bytes, info->wlen, cudaMemcpyDeviceToHost, c->st)); c->d2h += info->wlen;
         CK(c, cudaStreamSynchronize(c->st));
     }
@@ -534,9 +552,9 @@ extern "C" int rbf_decompress_mask(rbf_ctx* c, const uint8_t* bitmap, uint64_t l
     const size_t big = n > l ? (n > wlen ? n : wlen) : (l > wlen ? l : wlen);
     void *d_bytes, *d_out, *d_bits, *d_pass, *d_wit, *d_small;
     int rc;
-    if ((rc = scratch_get(c, 0, big, &d_bytes)) || (rc = scratch_get(c, 3, mw * 4, &d_out)) ||
-        (rc = scratch_get(c, 4, lw * 4, &d_bits)) || (rc = scratch_get(c, 5, pw * 4, &d_pass)) ||
-        (rc = scratch_get(c, 6, ww * 4, &d_wit)) || (rc = scratch_get(c, 7, 4096, &d_small)))
+    if ((rc = scratch_get(c, kScrBytes, big, &d_bytes)) || (rc = scratch_get(c, kScrMask, mw * 4, &d_out)) ||
+        (rc = scratch_get(c, kScrBits, lw * 4, &d_bits)) || (rc = scratch_get(c, kScrPass, pw * 4, &d_pass)) ||
+        (rc = scratch_get(c, kScrWit, ww * 4, &d_wit)) || (rc = scratch_get(c, kScrSmall, 4096, &d_small)))
         return rc;
     uint32_t* d_cnt = (uint32_t*)d_small;
     uint32_t* d_prefix = d_cnt + 4;
@@ -545,25 +563,20 @@ extern "C" int rbf_decompress_mask(rbf_ctx* c, const uint8_t* bitmap, uint64_t l
     CK(c, cudaMemsetAsync(d_wit, 0, ww * 4, c->st));
     CK(c, cudaMemsetAsync(d_out, 0, mw * 4, c->st));
     CK(c, cudaMemcpyAsync(d_bytes, bitmap, l, cudaMemcpyHostToDevice, c->st)); c->h2d += l;
-    LAUNCH(c, launch_pack_bytes((const uint8_t*)d_bytes, (uint32_t*)d_bits, l, c->sm_count, c->st));
+    CK(c, launch_pack_bytes(c->L, (const uint8_t*)d_bytes, (uint32_t*)d_bits, l, c->st));
     if (wlen) {
         CK(c, cudaMemcpyAsync(d_bytes, witness, wlen, cudaMemcpyHostToDevice, c->st)); c->h2d += wlen;
         // witness values are used as bits: any non-zero byte other than 1 is not representable; the reference
         // stores whatever the list holds (ivc:303); np.unpackbits output is 0/1 (ivc:1001-1002)
-        LAUNCH(c, launch_pack_bytes((const uint8_t*)d_bytes, (uint32_t*)d_wit, wlen, c->sm_count, c->st));
+        CK(c, launch_pack_bytes(c->L, (const uint8_t*)d_bytes, (uint32_t*)d_wit, wlen, c->st));
     }
-    FrameJob J; memset(&J, 0, sizeof J);
-    J.n = (uint32_t)n;
-    job_set_filter(J, l, k, *sd);
-    J.bits = (uint32_t*)d_bits; J.pass = (uint32_t*)d_pass; J.witness = (uint32_t*)d_wit; J.out_mask = (uint32_t*)d_out;
+    FrameJob J = frame_job(n, l, k, *sd, (uint32_t*)d_bits, (uint32_t*)d_wit, (uint32_t*)d_pass);
+    J.out_mask = (uint32_t*)d_out;
     J.wlen_in = (uint32_t)wlen;
     const uint32_t ncent = (uint32_t)((n + 99) / 100);
-    uint32_t h_prefix[2] = {0, ncent};
-    CK(c, cudaMemcpyAsync(d_job, &J, sizeof J, cudaMemcpyHostToDevice, c->st));
-    CK(c, cudaMemcpyAsync(d_prefix, h_prefix, 8, cudaMemcpyHostToDevice, c->st));
-    LAUNCH(c, launch_query(d_job, d_prefix, 1, ncent, (uint32_t)l, c->query_variant, c->sm_count, c->query_smem_cap, c->query_warps, c->st));
-    LAUNCH(c, launch_expand(d_job, 1, ncent, c->sm_count, (uint32_t*)((uint8_t*)d_small + 1024), d_cnt, c->st)); c->launches += 1;
-    LAUNCH(c, launch_unpack_bits((const uint32_t*)d_out, (uint8_t*)d_bytes, n, c->sm_count, c->st));
+    const uint32_t h_prefix[2] = {0, ncent};
+    if (int r = decode_enqueue(c, &J, d_job, h_prefix, d_prefix, 1, (uint32_t)l, ncent, (uint32_t*)((uint8_t*)d_small + 1024), d_cnt)) return r;
+    CK(c, launch_unpack_bits(c->L, (const uint32_t*)d_out, (uint8_t*)d_bytes, n, c->st));
     uint32_t h_cnt = 0;
     CK(c, cudaMemcpyAsync(out, d_bytes, n, cudaMemcpyDeviceToHost, c->st)); c->d2h += n;
     CK(c, cudaMemcpyAsync(&h_cnt, d_cnt, 4, cudaMemcpyDeviceToHost, c->st));
@@ -598,7 +611,8 @@ struct rbf_stream {
     int gray_mode = 0;      // 1: the mask is taken on cv2.COLOR_BGR2GRAY of the pixel (ivc:792-795) instead of on sample 0
     int value_mode = 0;     // changed-value gathers: 0 the current samples; 1 residuals (curr - prev) mod 2^(8 S) per sample
     bool last_k1_only = false;
-    size_t bits_hwm = 0, wit_hwm = 0;   // bytes per slot that may hold set bits (see stream_clear_outputs)
+    rbf_seeds last_sd = {};                 // seeds of the last encode (decode_verify rebuilds its jobs from them and last_infos)
+    size_t bits_hwm = 0, wit_hwm = 0;   // bytes per slot that may hold set bits (see enc_stage_jobs)
     bool wit_dirty_full = false;
     std::vector<cudaEvent_t> ev_copy;
     std::vector<rbf_mask_info> last_infos;
@@ -706,31 +720,30 @@ extern "C" int rbf_stream_bitmap_region(rbf_stream* s, void** dptr, uint64_t* st
     return RBF_OK;
 }
 
-// `diff > threshold` with integer diff and a Python float threshold (ivc:808)  ==  diff > floor(threshold)
-static int threshold_to_int(double thr) {
+// `diff > threshold` with integer diff and a Python float threshold (ivc:808)  ==  diff > floor(threshold).  The int16 abs of 16-bit
+// samples can be -32768 (ivc:801), so for them a threshold below -1 keeps its exact floor (down to -40000).
+static int threshold_to_int(double thr, uint32_t sample_bytes) {
     if (isnan(thr)) return 0x7fffffff;                 // every comparison with NaN is False
-    if (thr < -1.0) return -1;                         // diff >= -32768 only for uint16 wrap; handled below
+    if (thr < -1.0) return sample_bytes == 2 ? (thr < -40000.0 ? -40000 : (int)floor(thr)) : -1;
     if (thr > 1e9) return 0x7fffffff;
     return (int)floor(thr);
 }
 
-// ---- pieces of the batched encode ----------------------------------------------------------
-static int stream_thr_int(const rbf_stream* s, double threshold) {
-    int thr_int = threshold_to_int(threshold);
-    if (s->S == 2 && threshold < -1.0)                  // int16 abs can be -32768 (ivc:801): keep exact floor
-        thr_int = threshold < -40000.0 ? -40000 : (int)floor(threshold);
-    return thr_int;
-}
-
-static int stream_fill_pairs(rbf_stream* s, uint32_t first, uint32_t count, const uint32_t* prev_idx, const uint32_t* curr_idx) {
+// ---- steps of the batched encode, shared by rbf_stream_encode and rbf_stream_encode_host ---------------------------------
+// The PairJobs of pairs [first, first+count) go to the device and their K1 counts are zeroed, on the context's stream.
+static int enc_stage_pairs(rbf_stream* s, uint32_t first, uint32_t count, const uint32_t* prev_idx, const uint32_t* curr_idx) {
+    rbf_ctx* c = s->c;
     for (uint32_t i = 0; i < count; i++) {
         if (prev_idx[i] >= s->max_frames || curr_idx[i] >= s->max_frames)
-            return set_err(s->c, RBF_ERR_INVALID, "pair %u references a frame outside the store", first + i);
+            return set_err(c, RBF_ERR_INVALID, "pair %u references a frame outside the store", first + i);
         PairJob& P = s->h_pairs[first + i];
         P.prev = s->d_frames + (size_t)prev_idx[i] * s->frame_stride;
         P.curr = s->d_frames + (size_t)curr_idx[i] * s->frame_stride;
         P.mask = s->d_mask + (size_t)(first + i) * s->mask_stride_w;
     }
+    CK(c, cudaMemcpyAsync(s->d_pairs + first, s->h_pairs + first, sizeof(PairJob) * count, cudaMemcpyHostToDevice, c->st));
+    CK(c, cudaMemsetAsync(s->d_ones + first, 0, 4 * (size_t)count, c->st));
+    CK(c, cudaMemsetAsync(s->d_resid + first, 0, 4 * (size_t)count, c->st));
     return RBF_OK;
 }
 
@@ -743,6 +756,28 @@ static bool pairs_form_chain(const PairJob* h, uint32_t count) {
         if (i + 1 < count && h[i].curr != h[i + 1].prev) return false;
     }
     return true;
+}
+
+// K1 over pairs [f, f+cnt) on `st`, then the copy of their counts to the host.  pipelined: K2 runs beside it.
+static int enc_k1(rbf_stream* s, uint32_t f, uint32_t cnt, int thr_int, bool pipelined, cudaStream_t st) {
+    rbf_ctx* c = s->c;
+    CK(c, launch_threshold(c->L, s->d_pairs + f, (int)cnt, (uint32_t)s->npix, (int)s->C, (int)s->S, thr_int, s->mask_mode, s->gray_mode,
+                           s->d_ones + f, s->d_resid + f, pairs_form_chain(s->h_pairs + f, cnt), pipelined, st));
+    CK(c, cudaMemcpyAsync(s->h_ones + f, s->d_ones + f, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, st));
+    CK(c, cudaMemcpyAsync(s->h_resid + f, s->d_resid + f, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, st));
+    c->d2h += 8 * (int64_t)cnt;
+    return RBF_OK;
+}
+
+// The FrameJob of pair slot i in h_jobs: the slot's bit array, witness and pass mask, and the filter of (l, k*) when l > 0.
+// out == NULL: an encode job over the slot's mask; otherwise a decode job writing `out` from a witness of wlen bits.
+static FrameJob& slot_job(rbf_stream* s, uint32_t i, uint64_t l, double k_star, const rbf_seeds& sd, uint32_t* out, uint64_t wlen) {
+    const size_t mw = (size_t)i * s->mask_stride_w;
+    FrameJob& J = s->h_jobs[i];
+    J = frame_job(s->npix, l, k_star, sd, s->d_bits + mw, s->d_wit + mw, s->d_pass + (size_t)i * s->pass_stride_w);
+    if (out) { J.out_mask = out; J.wlen_in = l ? (uint32_t)wlen : 0u; }
+    else J.mask = s->d_mask + mw;
+    return J;
 }
 
 struct RangeTotals {
@@ -765,15 +800,8 @@ static void stream_range_params(rbf_stream* s, uint32_t first, uint32_t count, c
         int coded = rbf_optimal_params(n, in.ones, &p, &k, &l);
         in.p = p;
         if (kov && kov[i] > 0.0 && !(p >= kPStar)) { k = kov[i]; l = lov ? lov[i] : 0; coded = !(l == 0 || l >= n); }
-        FrameJob& J = s->h_jobs[first + i];
-        memset(&J, 0, sizeof J);
-        J.n = n;
-        J.mask = s->d_mask + (size_t)(first + i) * s->mask_stride_w;
-        J.bits = s->d_bits + (size_t)(first + i) * s->mask_stride_w;
-        J.witness = s->d_wit + (size_t)(first + i) * s->mask_stride_w;
-        J.pass = s->d_pass + (size_t)(first + i) * s->pass_stride_w;
+        const FrameJob& J = slot_job(s, first + i, coded ? l : 0, k, *sd, nullptr, 0);
         if (coded) {
-            job_set_filter(J, l, k, *sd);
             in.k = k; in.l = l; in.floor_k = J.floor_k; in.act_T = J.act_T;
             total_cent += ncent; out->coded_pairs++;
             if (l > out->max_l) out->max_l = (uint32_t)l;
@@ -785,73 +813,85 @@ static void stream_range_params(rbf_stream* s, uint32_t first, uint32_t count, c
     out->total_cent = total_cent - base_cent;
 }
 
-// Zero what K2 / K3b will OR into.  Nothing ever writes a bit array at or beyond bit l, or a witness at or beyond bit wlen,
-// and both regions are fully zeroed at creation, so clearing [0, high-water mark) of every slot is enough.
-static int stream_clear_outputs(rbf_stream* s, uint32_t first, uint32_t count, uint32_t max_l, cudaStream_t st) {
+// The FrameJobs of pairs [f, f+cnt) go to the device, with their work list hp (cnt + 1 entries inside h_prefix, or NULL), then what
+// K2 / K3b will OR into is zeroed, once the slot packing of a pending all-gather has read the bit arrays.  Nothing ever writes a bit
+// array at or beyond bit l, or a witness at or beyond bit wlen, and both regions are fully zeroed at creation, so clearing
+// [0, high-water mark) of every slot is enough.  Keep the work list behind the jobs: uploaded ahead of them, it held K2 of
+// rbf_stream_encode_host's first chunk until every frame copy of the call had landed (+20 ms per 4K call on an H100 at 700 W).
+static int enc_stage_jobs(rbf_stream* s, uint32_t f, uint32_t cnt, uint32_t max_l, const uint32_t* hp) {
     rbf_ctx* c = s->c;
+    CK(c, cudaMemcpyAsync(s->d_jobs + f, s->h_jobs + f, sizeof(FrameJob) * cnt, cudaMemcpyHostToDevice, c->st));
+    if (hp) CK(c, cudaMemcpyAsync(s->d_prefix + (hp - s->h_prefix), hp, 4 * ((size_t)cnt + 1), cudaMemcpyHostToDevice, c->st));
+    if (int r = wait_pack(c)) return r;
     const size_t stride = s->mask_stride_w * 4;
     const size_t need = align_up((size_t)((max_l + 31u) / 32u) * 4 + 64, 128);
     if (need > s->bits_hwm) s->bits_hwm = need;
     const size_t wb = s->bits_hwm < stride ? s->bits_hwm : stride;
     const size_t ww = (s->wit_dirty_full || s->wit_hwm > stride) ? stride : s->wit_hwm;
-    CK(c, cudaMemset2DAsync(s->d_bits + (size_t)first * s->mask_stride_w, stride, 0, wb, count, st));
-    if (ww) CK(c, cudaMemset2DAsync(s->d_wit + (size_t)first * s->mask_stride_w, stride, 0, ww, count, st));
+    CK(c, cudaMemset2DAsync(s->d_bits + (size_t)f * s->mask_stride_w, stride, 0, wb, cnt, c->st));
+    if (ww) CK(c, cudaMemset2DAsync(s->d_wit + (size_t)f * s->mask_stride_w, stride, 0, ww, cnt, c->st));
     return RBF_OK;
 }
-static void stream_note_witness(rbf_stream* s, uint32_t first, uint32_t count) {      // after the encode has been synchronised
-    for (uint32_t i = 0; i < count; i++) {
-        const size_t nb = align_up((size_t)((s->h_wlen[first + i] + 31u) / 32u) * 4 + 64, 128);
-        if (nb > s->wit_hwm) s->wit_hwm = nb;
+
+// K3b over pairs [f, f+cnt) and the copy of their witness lengths to the host.  timed: the last two stage events bracket K3b,
+// which completes the stage timings of rbf_stream_stage_ms.
+static int enc_witness(rbf_stream* s, uint32_t f, uint32_t cnt, bool timed) {
+    rbf_ctx* c = s->c;
+    if (timed) CK(c, cudaEventRecord(s->ev[4], c->st));
+    s->wit_dirty_full = true;                            // until the witness lengths of this encode are known
+    CK(c, launch_witness(c->L, s->d_jobs + f, (int)cnt, (uint32_t)((s->npix + 99) / 100), s->d_chunkcnt + 32 * (size_t)f, s->d_wlen + f,
+                         c->st));
+    if (timed) { CK(c, cudaEventRecord(s->ev[5], c->st)); s->staged = true; }
+    CK(c, cudaMemcpyAsync(s->h_wlen + f, s->d_wlen + f, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, c->st));
+    c->d2h += 4 * (int64_t)cnt;
+    return RBF_OK;
+}
+
+// An encode starts: the slots hold no complete encode (fetch, gather and decode_verify refuse) until enc_finish.
+static void enc_begin(rbf_stream* s, const rbf_seeds* sd) {
+    s->last_infos.clear();
+    s->last_pairs = 0; s->last_max_l = 0;
+    s->staged = false;
+    s->last_sd = *sd;
+}
+
+// After the encode of pairs [0, pairs) has been synchronised: what fetch, gather and decode_verify read, the witness high-water
+// mark of the next encode's clear, and the caller's infos.
+static void enc_finish(rbf_stream* s, uint32_t pairs, rbf_mask_info* infos) {
+    const bool coded_run = !s->k1_only;
+    s->last_pairs = pairs;
+    s->last_k1_only = !coded_run;
+    if (coded_run) {
+        for (uint32_t i = 0; i < pairs; i++) {
+            const size_t nb = align_up((size_t)((s->h_wlen[i] + 31u) / 32u) * 4 + 64, 128);
+            if (nb > s->wit_hwm) s->wit_hwm = nb;
+        }
+        s->wit_dirty_full = false;
+    }
+    for (uint32_t i = 0; i < pairs; i++) {
+        rbf_mask_info& in = s->last_infos[i];
+        if (!in.raw && in.l > s->last_max_l) s->last_max_l = (uint32_t)in.l;
+        if (coded_run && !in.raw) in.wlen = s->h_wlen[i];
+        if (infos) infos[i] = in;
     }
 }
 
-// Encode pairs [first, first+count) (slots of all per-pair arrays) serially on the context's stream; `pfx` is the slot of this
-// range's century-prefix array (count+1 entries) inside h_prefix/d_prefix.  Used per chunk by rbf_stream_encode_host.
+// Encode pairs [first, first+count) serially on the context's stream (one chunk of rbf_stream_encode_host); `pfx` is the slot of this
+// range's century-prefix array (count+1 entries) inside h_prefix/d_prefix.
 static int stream_encode_range(rbf_stream* s, uint32_t first, uint32_t count, uint32_t pfx, const uint32_t* prev_idx,
-                               const uint32_t* curr_idx, double threshold, const rbf_seeds* sd, const double* kov,
-                               const uint64_t* lov, bool record_events) {
+                               const uint32_t* curr_idx, int thr_int, const rbf_seeds* sd) {
     rbf_ctx* c = s->c;
-    const uint32_t n = (uint32_t)s->npix;
-    const int thr_int = stream_thr_int(s, threshold);
-    if (int r = stream_fill_pairs(s, first, count, prev_idx, curr_idx)) return r;
-    CK(c, cudaMemcpyAsync(s->d_pairs + first, s->h_pairs + first, sizeof(PairJob) * count, cudaMemcpyHostToDevice, c->st));
-    CK(c, cudaMemsetAsync(s->d_ones + first, 0, 4 * (size_t)count, c->st));
-    CK(c, cudaMemsetAsync(s->d_resid + first, 0, 4 * (size_t)count, c->st));
-    if (record_events) { s->staged = false; CK(c, cudaEventRecord(s->ev[0], c->st)); }
-    LAUNCH(c, launch_threshold(s->d_pairs + first, (int)count, n, (int)s->C, (int)s->S, thr_int, s->mask_mode, s->gray_mode,
-                               s->d_ones + first, s->d_resid + first, c->k1_variant, pairs_form_chain(s->h_pairs + first, count),
-                               c->sm_count, c->k1_ctas_per_sm, c->st));
-    if (c->k1_variant == 1 && !s->gray_mode) c->launches++;              // tail kernel
-    if (record_events) CK(c, cudaEventRecord(s->ev[1], c->st));
-    CK(c, cudaMemcpyAsync(s->h_ones + first, s->d_ones + first, 4 * (size_t)count, cudaMemcpyDeviceToHost, c->st));
-    CK(c, cudaMemcpyAsync(s->h_resid + first, s->d_resid + first, 4 * (size_t)count, cudaMemcpyDeviceToHost, c->st));
-    c->d2h += 8 * (int64_t)count;
+    if (int r = enc_stage_pairs(s, first, count, prev_idx, curr_idx)) return r;
+    if (int r = enc_k1(s, first, count, thr_int, false, c->st)) return r;
     CK(c, cudaStreamSynchronize(c->st));               // the one host round trip: (p, k, l, T) need libm's log2
-    const uint32_t ncent = (n + 99u) / 100u;
     RangeTotals rt;
     uint32_t* hp = s->h_prefix + pfx;
-    stream_range_params(s, first, count, sd, kov, lov, hp, 0, &rt);
-    if (first + count > s->last_pairs || first == 0) s->last_pairs = first + count;
-    if (rt.max_l > s->last_max_l || first == 0) s->last_max_l = rt.max_l;
-    s->last_k1_only = s->k1_only != 0;
-    if (rt.coded_pairs == 0 || s->k1_only) return RBF_OK;
-    CK(c, cudaMemcpyAsync(s->d_jobs + first, s->h_jobs + first, sizeof(FrameJob) * count, cudaMemcpyHostToDevice, c->st));
-    CK(c, cudaMemcpyAsync(s->d_prefix + pfx, hp, 4 * ((size_t)count + 1), cudaMemcpyHostToDevice, c->st));
-    if (int r = wait_pack(c)) return r;                  // the slots of the last all-gather are packed
-    if (int r = stream_clear_outputs(s, first, count, rt.max_l, c->st)) return r;
-    if (record_events) CK(c, cudaEventRecord(s->ev[2], c->st));
-    LAUNCH(c, launch_insert(s->d_jobs + first, (int)count, ncent, rt.max_l, c->insert_variant, c->sm_count, c->k2_clusters, c->st));
-    if (record_events) CK(c, cudaEventRecord(s->ev[3], c->st));
-    LAUNCH(c, launch_query(s->d_jobs + first, s->d_prefix + pfx, (int)count, rt.total_cent, rt.max_l, c->query_variant, c->sm_count,
-                           c->query_smem_cap, c->query_warps, c->st));
-    if (record_events) CK(c, cudaEventRecord(s->ev[4], c->st));
-    s->wit_dirty_full = true;                            // until the witness lengths of this encode are known
-    LAUNCH(c, launch_witness(s->d_jobs + first, (int)count, ncent, c->sm_count, s->d_chunkcnt + 32 * (size_t)first, s->d_wlen + first, c->st));
-    c->launches += 2;                                   // pass-count + finalize kernels
-    if (record_events) { CK(c, cudaEventRecord(s->ev[5], c->st)); s->staged = true; }
-    CK(c, cudaMemcpyAsync(s->h_wlen + first, s->d_wlen + first, 4 * (size_t)count, cudaMemcpyDeviceToHost, c->st));
-    c->d2h += 4 * (int64_t)count;
-    return RBF_OK;
+    stream_range_params(s, first, count, sd, nullptr, nullptr, hp, 0, &rt);
+    if (rt.coded_pairs == 0) return RBF_OK;
+    if (int r = enc_stage_jobs(s, first, count, rt.max_l, hp)) return r;
+    CK(c, launch_insert(c->L, s->d_jobs + first, (int)count, (uint32_t)((s->npix + 99) / 100), rt.max_l, c->st));
+    CK(c, launch_query(c->L, s->d_jobs + first, s->d_prefix + pfx, (int)count, rt.total_cent, rt.max_l, c->st));
+    return enc_witness(s, first, count, false);
 }
 
 static int ensure_pipe_streams(rbf_ctx* c) {
@@ -871,37 +911,24 @@ static int ensure_pipe_streams(rbf_ctx* c) {
 static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t* prev_idx, const uint32_t* curr_idx,
                                    double threshold, const rbf_seeds* sd, const double* kov, const uint64_t* lov) {
     rbf_ctx* c = s->c;
-    const uint32_t n = (uint32_t)s->npix, ncent = (n + 99u) / 100u;
-    const int thr_int = stream_thr_int(s, threshold);
+    const uint32_t ncent = (uint32_t)((s->npix + 99) / 100);
+    const int thr_int = threshold_to_int(threshold, s->S);
     uint32_t R = (uint32_t)c->encode_ranges;
     if (R > 8u) R = 8u;
     if (pairs < 8u * R) R = 1u;                          // small jobs: nothing to hide behind
     if (int r = ensure_pipe_streams(c)) return r;
-    if (int r = stream_fill_pairs(s, 0, pairs, prev_idx, curr_idx)) return r;
-    CK(c, cudaMemcpyAsync(s->d_pairs, s->h_pairs, sizeof(PairJob) * pairs, cudaMemcpyHostToDevice, c->st));
-    CK(c, cudaMemsetAsync(s->d_ones, 0, 4 * (size_t)pairs, c->st));
-    CK(c, cudaMemsetAsync(s->d_resid, 0, 4 * (size_t)pairs, c->st));
-    s->staged = false;
+    if (int r = enc_stage_pairs(s, 0, pairs, prev_idx, curr_idx)) return r;
+    enc_begin(s, sd);
     CK(c, cudaEventRecord(s->ev[0], c->st));
     CK(c, cudaEventRecord(c->ev_fork, c->st));
     CK(c, cudaStreamWaitEvent(c->st_k1, c->ev_fork, 0));
     uint32_t lo[9];
     for (uint32_t r = 0; r <= R; r++) lo[r] = (uint32_t)(((uint64_t)pairs * r) / R);
-    const int k1_cap = R > 1u ? c->pipe_k1_ctas_per_sm : c->k1_ctas_per_sm;
     for (uint32_t r = 0; r < R; r++) {
-        const uint32_t f = lo[r], cnt = lo[r + 1] - lo[r];
-        LAUNCH(c, launch_threshold(s->d_pairs + f, (int)cnt, n, (int)s->C, (int)s->S, thr_int, s->mask_mode, s->gray_mode, s->d_ones + f,
-                                   s->d_resid + f, c->k1_variant, pairs_form_chain(s->h_pairs + f, cnt), c->sm_count, k1_cap, c->st_k1));
-        if (c->k1_variant == 1 && !s->gray_mode) c->launches++;
-        CK(c, cudaMemcpyAsync(s->h_ones + f, s->d_ones + f, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, c->st_k1));
-        CK(c, cudaMemcpyAsync(s->h_resid + f, s->d_resid + f, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, c->st_k1));
+        if (int e = enc_k1(s, lo[r], lo[r + 1] - lo[r], thr_int, R > 1u, c->st_k1)) return e;
         CK(c, cudaEventRecord(c->ev_k1[r], c->st_k1));
     }
     CK(c, cudaEventRecord(s->ev[1], c->st_k1));           // end of the last K1
-    c->d2h += 8 * (int64_t)pairs;
-    s->last_infos.clear();
-    s->last_pairs = pairs; s->last_max_l = 0;
-    s->last_k1_only = s->k1_only != 0;
     RangeTotals all;
     uint32_t base_cent = 0;
     bool first_k2 = true;
@@ -922,14 +949,10 @@ static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t
         if (rt.max_l > all.max_l) all.max_l = rt.max_l;
         if (s->k1_only || rt.coded_pairs == 0) continue;
         CK(c, cudaStreamWaitEvent(c->st, c->ev_k1[r], 0)); // K2 reads the masks K1 wrote on the other stream
-        CK(c, cudaMemcpyAsync(s->d_jobs + f, s->h_jobs + f, sizeof(FrameJob) * cnt, cudaMemcpyHostToDevice, c->st));
-        if (first_k2) { if (int e = wait_pack(c)) return e; }
-        if (int e = stream_clear_outputs(s, f, cnt, rt.max_l, c->st)) return e;
+        if (int e = enc_stage_jobs(s, f, cnt, rt.max_l, nullptr)) return e;   // the work list goes up once, for all ranges
         if (first_k2) { CK(c, cudaEventRecord(s->ev[2], c->st)); first_k2 = false; }
-        if (!kq) LAUNCH(c, launch_insert(s->d_jobs + f, (int)cnt, ncent, rt.max_l, c->insert_variant, c->sm_count, c->k2_clusters, c->st));
+        if (!kq) CK(c, launch_insert(c->L, s->d_jobs + f, (int)cnt, ncent, rt.max_l, c->st));
     }
-    all.total_cent = base_cent;
-    s->last_max_l = all.max_l;
     if (s->k1_only || all.coded_pairs == 0) {
         CK(c, cudaStreamWaitEvent(c->st, c->ev_k1[R - 1], 0));
         return RBF_OK;
@@ -938,7 +961,7 @@ static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t
     if (kq) {
         uint32_t qlo[9];
         for (uint32_t q = 0; q <= Q; q++) qlo[q] = (uint32_t)(((uint64_t)pairs * q) / Q);
-        // per-range work lists for K3 (each starts at 0), behind the whole-encode list that decode_verify uses
+        // per-range work lists for K3 (each starts at 0), behind the whole-encode list
         uint32_t* hp2 = s->h_prefix + pairs + 1;
         uint32_t off = 0, range_cent[8], range_off[8];
         for (uint32_t q = 0; q < Q; q++) {
@@ -952,27 +975,17 @@ static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t
         CK(c, cudaStreamWaitEvent(c->st_k1, c->ev_fork, 0));
         for (uint32_t q = 0; q < Q; q++) {
             const uint32_t f = qlo[q], cnt = qlo[q + 1] - qlo[q];
-            LAUNCH(c, launch_insert(s->d_jobs + f, (int)cnt, ncent, all.max_l, c->insert_variant, c->sm_count, c->k2_clusters, c->st_k1));
+            CK(c, launch_insert(c->L, s->d_jobs + f, (int)cnt, ncent, all.max_l, c->st_k1));
             CK(c, cudaEventRecord(c->ev_k1[q], c->st_k1));
             CK(c, cudaStreamWaitEvent(c->st, c->ev_k1[q], 0));
             if (q == 0) CK(c, cudaEventRecord(s->ev[3], c->st));
-            LAUNCH(c, launch_query(s->d_jobs + f, s->d_prefix + pairs + 1 + range_off[q], (int)cnt, range_cent[q], all.max_l, c->query_variant,
-                                   c->sm_count, c->query_smem_cap, c->query_warps, c->st));
+            CK(c, launch_query(c->L, s->d_jobs + f, s->d_prefix + pairs + 1 + range_off[q], (int)cnt, range_cent[q], all.max_l, c->st));
         }
     } else {
         CK(c, cudaEventRecord(s->ev[3], c->st));
-        LAUNCH(c, launch_query(s->d_jobs, s->d_prefix, (int)pairs, all.total_cent, all.max_l, c->query_variant, c->sm_count,
-                               c->query_smem_cap, c->query_warps, c->st));
+        CK(c, launch_query(c->L, s->d_jobs, s->d_prefix, (int)pairs, base_cent, all.max_l, c->st));
     }
-    CK(c, cudaEventRecord(s->ev[4], c->st));
-    s->wit_dirty_full = true;
-    LAUNCH(c, launch_witness(s->d_jobs, (int)pairs, ncent, c->sm_count, s->d_chunkcnt, s->d_wlen, c->st));
-    c->launches += 2;                                   // pass-count + finalize kernels
-    CK(c, cudaEventRecord(s->ev[5], c->st));
-    s->staged = true;
-    CK(c, cudaMemcpyAsync(s->h_wlen, s->d_wlen, 4 * (size_t)pairs, cudaMemcpyDeviceToHost, c->st));
-    c->d2h += 4 * (int64_t)pairs;
-    return RBF_OK;
+    return enc_witness(s, 0, pairs, true);
 }
 
 extern "C" int rbf_stream_encode(rbf_stream* s, const uint32_t* prev_idx, const uint32_t* curr_idx, uint32_t pairs,
@@ -985,12 +998,7 @@ extern "C" int rbf_stream_encode(rbf_stream* s, const uint32_t* prev_idx, const 
     int rc = stream_encode_pipelined(s, pairs, prev_idx, curr_idx, threshold, sd, kov, lov);
     if (rc) { cudaStreamSynchronize(c->st_k1); cudaStreamSynchronize(c->st); return rc; }
     CK(c, cudaStreamSynchronize(c->st));
-    const bool coded_run = !s->k1_only;
-    if (coded_run) { stream_note_witness(s, 0, pairs); s->wit_dirty_full = false; }
-    for (uint32_t i = 0; i < pairs; i++) {
-        s->last_infos[i].wlen = (coded_run && !s->last_infos[i].raw) ? s->h_wlen[i] : 0;
-        if (infos) infos[i] = s->last_infos[i];
-    }
+    enc_finish(s, pairs, infos);
     return RBF_OK;
 }
 
@@ -1023,6 +1031,16 @@ extern "C" int rbf_stream_fetch(rbf_stream* s, uint32_t pair, uint8_t* bitmap, u
     return RBF_OK;
 }
 
+// Pairs [first, first+count) of a per-pair device region into host rows of `slot` bytes, row 0 for pair `first` (a row takes what fits
+// of its pair's slot); no copy when host is NULL or slot is 0.
+static int copy_slots_d2h(rbf_stream* s, uint8_t* host, uint64_t slot, const uint32_t* region, uint32_t first, uint32_t count, cudaStream_t st) {
+    if (!host || !slot) return RBF_OK;
+    const size_t stride = s->mask_stride_w * 4, w = slot < stride ? (size_t)slot : stride;
+    CK(s->c, cudaMemcpy2DAsync(host, slot, (const uint8_t*)region + (size_t)first * stride, stride, w, count, cudaMemcpyDeviceToHost, st));
+    s->c->d2h += (int64_t)w * count;
+    return RBF_OK;
+}
+
 // One strided copy per output kind for pairs [first, first+count) and ONE synchronisation (the GOP loop's batched fetch).
 extern "C" int rbf_stream_fetch_batch(rbf_stream* s, uint32_t first, uint32_t count, uint8_t* bitmaps, uint64_t bitmap_slot,
                                       uint8_t* witness, uint64_t witness_slot, uint8_t* masks_little, uint64_t mask_slot) {
@@ -1031,15 +1049,11 @@ extern "C" int rbf_stream_fetch_batch(rbf_stream* s, uint32_t first, uint32_t co
     if (count == 0 || (uint64_t)first + count > s->last_pairs) return set_err(c, RBF_ERR_INVALID, "pairs [%u,%u) were not encoded", first, first + count);
     if (s->last_k1_only && (bitmaps || witness))
         return set_err(c, RBF_ERR_STATE, "the last encode stopped after K1 (k1_only): there is no bitmap / witness to fetch");
-    const size_t stride = s->mask_stride_w * 4;
-    auto copy2d = [&](uint8_t* dst, uint64_t slot, const uint32_t* src) -> cudaError_t {
-        const size_t w = slot < stride ? (size_t)slot : stride;
-        c->d2h += (int64_t)w * count;
-        return cudaMemcpy2DAsync(dst, slot, (const uint8_t*)src + (size_t)first * stride, stride, w, count, cudaMemcpyDeviceToHost, c->st);
-    };
-    if (bitmaps && bitmap_slot) CK(c, copy2d(bitmaps, bitmap_slot, s->d_bits));
-    if (witness && witness_slot) CK(c, copy2d(witness, witness_slot, s->d_wit));
-    if (masks_little && mask_slot) CK(c, copy2d(masks_little, mask_slot, s->d_mask));
+    int r;
+    if ((r = copy_slots_d2h(s, bitmaps, bitmap_slot, s->d_bits, first, count, c->st)) ||
+        (r = copy_slots_d2h(s, witness, witness_slot, s->d_wit, first, count, c->st)) ||
+        (r = copy_slots_d2h(s, masks_little, mask_slot, s->d_mask, first, count, c->st)))
+        return r;
     CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
 }
@@ -1068,9 +1082,8 @@ extern "C" int rbf_stream_encode_host(rbf_stream* s, const void* host_frames, ui
         CK(c, cudaEventRecord(s->ev_copy[k], c->st_copy));
     }
     c->h2d += (int64_t)s->frame_bytes * nframes;
-    s->last_infos.clear();
-    s->last_pairs = 0; s->last_max_l = 0;
-    const size_t stride = s->mask_stride_w * 4;
+    enc_begin(s, sd);
+    const int thr_int = threshold_to_int(threshold, s->S);
     std::vector<uint32_t> pi, ci;
     for (uint32_t k = 0; k < nchunks; k++) {
         const uint32_t f0 = k * CH, f1 = (f0 + CH < nframes) ? f0 + CH : nframes;
@@ -1080,42 +1093,19 @@ extern "C" int rbf_stream_encode_host(rbf_stream* s, const void* host_frames, ui
         pi.resize(cnt); ci.resize(cnt);
         for (uint32_t i = 0; i < cnt; i++) { pi[i] = p0 + i; ci[i] = p0 + i + 1; }
         CK(c, cudaStreamWaitEvent(c->st, s->ev_copy[k], 0));
-        int rc = stream_encode_range(s, p0, cnt, p0 + k, pi.data(), ci.data(), threshold, sd, nullptr, nullptr, false);
-        if (rc) return rc;
+        if (int rc = stream_encode_range(s, p0, cnt, p0 + k, pi.data(), ci.data(), thr_int, sd)) return rc;
         // the packed results of this chunk go back on their own stream, beside the kernels of the next chunk
         CK(c, cudaEventRecord(c->ev_d2h, c->st));
         CK(c, cudaStreamWaitEvent(c->st_d2h, c->ev_d2h, 0));
-        if (bitmaps && bitmap_slot) {
-            const size_t w = bitmap_slot < stride ? bitmap_slot : stride;
-            CK(c, cudaMemcpy2DAsync(bitmaps + (size_t)p0 * bitmap_slot, bitmap_slot, (const uint8_t*)s->d_bits + (size_t)p0 * stride, stride,
-                                    w, cnt, cudaMemcpyDeviceToHost, c->st_d2h));
-            c->d2h += (int64_t)w * cnt;
-        }
-        if (witness && witness_slot) {
-            const size_t w = witness_slot < stride ? witness_slot : stride;
-            CK(c, cudaMemcpy2DAsync(witness + (size_t)p0 * witness_slot, witness_slot, (const uint8_t*)s->d_wit + (size_t)p0 * stride, stride,
-                                    w, cnt, cudaMemcpyDeviceToHost, c->st_d2h));
-            c->d2h += (int64_t)w * cnt;
-        }
+        int r;
+        if ((r = copy_slots_d2h(s, bitmaps ? bitmaps + (size_t)p0 * bitmap_slot : nullptr, bitmap_slot, s->d_bits, p0, cnt, c->st_d2h)) ||
+            (r = copy_slots_d2h(s, witness ? witness + (size_t)p0 * witness_slot : nullptr, witness_slot, s->d_wit, p0, cnt, c->st_d2h)))
+            return r;
     }
     CK(c, cudaEventRecord(c->ev_d2h, c->st_d2h));        // the caller's timer / next call on `st` sees the copies done
     CK(c, cudaStreamWaitEvent(c->st, c->ev_d2h, 0));
     CK(c, cudaStreamSynchronize(c->st));
-    stream_note_witness(s, 0, pairs);
-    s->wit_dirty_full = false;
-    // one contiguous prefix array for later decode_verify over all pairs
-    {
-        const uint32_t ncent = (uint32_t)((s->npix + 99) / 100);
-        uint32_t tot = 0;
-        s->h_prefix[0] = 0;
-        for (uint32_t i = 0; i < pairs; i++) { if (!s->last_infos[i].raw) tot += ncent; s->h_prefix[i + 1] = tot; }
-        CK(c, cudaMemcpyAsync(s->d_prefix, s->h_prefix, 4 * ((size_t)pairs + 1), cudaMemcpyHostToDevice, c->st));
-        CK(c, cudaStreamSynchronize(c->st));
-    }
-    for (uint32_t i = 0; i < pairs; i++) {
-        if (!s->last_infos[i].raw) s->last_infos[i].wlen = s->h_wlen[i];
-        if (infos) infos[i] = s->last_infos[i];
-    }
+    enc_finish(s, pairs, infos);
     return RBF_OK;
 }
 
@@ -1129,25 +1119,24 @@ extern "C" int rbf_stream_decode_verify(rbf_stream* s, uint32_t pairs, uint64_t*
     CK(c, cudaMemsetAsync(s->d_dec, 0, stride_w * 4 * pairs, c->st));
     // bitmap and witness sit in packbits order after K3b; the kernels work LSB-first
     if (int r = wait_pack(c)) return r;
-    LAUNCH(c, launch_bitrev(s->d_bits, stride_w * pairs, c->sm_count, c->st));
-    LAUNCH(c, launch_bitrev(s->d_wit, stride_w * pairs, c->sm_count, c->st));
+    CK(c, launch_bitrev(c->L, s->d_bits, stride_w * pairs, c->st));
+    CK(c, launch_bitrev(c->L, s->d_wit, stride_w * pairs, c->st));
+    // the decode jobs and their work list come from what the encode stored; a real decode knows no mask (ivc:286-304)
+    const uint32_t ncent = (uint32_t)((s->npix + 99) / 100);
+    s->h_prefix[0] = 0;
     for (uint32_t i = 0; i < pairs; i++) {
-        FrameJob& J = s->h_jobs[i];
-        J.out_mask = s->d_dec + (size_t)i * stride_w;
-        J.wlen_in = (uint32_t)s->last_infos[i].wlen;
-        J.mask = nullptr;                               // a real decode knows no mask (ivc:286-304)
+        const rbf_mask_info& in = s->last_infos[i];
+        slot_job(s, i, in.raw ? 0 : in.l, in.k, s->last_sd, s->d_dec + (size_t)i * stride_w, in.wlen);
+        s->h_prefix[i + 1] = s->h_prefix[i] + (in.raw ? 0 : ncent);
     }
-    CK(c, cudaMemcpyAsync(s->d_jobs, s->h_jobs, sizeof(FrameJob) * pairs, cudaMemcpyHostToDevice, c->st));
-    const uint32_t total_cent = s->h_prefix[pairs];
-    LAUNCH(c, launch_query(s->d_jobs, s->d_prefix, (int)pairs, total_cent, s->last_max_l, c->query_variant, c->sm_count, c->query_smem_cap, c->query_warps, c->st));
-    LAUNCH(c, launch_expand(s->d_jobs, (int)pairs, (uint32_t)((s->npix + 99) / 100), c->sm_count, s->d_chunkcnt, s->d_wlen, c->st));
-    c->launches += 1;
+    if (int r = decode_enqueue(c, s->h_jobs, s->d_jobs, s->h_prefix, s->d_prefix, (int)pairs, s->last_max_l, ncent, s->d_chunkcnt, s->d_wlen))
+        return r;
     void* d_cnt; int rc;
-    if ((rc = scratch_get(c, 7, 4 * (size_t)pairs + 4096, &d_cnt))) return rc;
+    if ((rc = scratch_get(c, kScrSmall, 4 * (size_t)pairs + 4096, &d_cnt))) return rc;
     CK(c, cudaMemsetAsync(d_cnt, 0, 4 * (size_t)pairs, c->st));
-    LAUNCH(c, launch_count_diff(s->d_mask, s->d_dec, stride_w, (s->npix + 31) / 32, (int)pairs, (uint32_t*)d_cnt, c->sm_count, c->st));
-    LAUNCH(c, launch_bitrev(s->d_bits, stride_w * pairs, c->sm_count, c->st));
-    LAUNCH(c, launch_bitrev(s->d_wit, stride_w * pairs, c->sm_count, c->st));
+    CK(c, launch_count_diff(c->L, s->d_mask, s->d_dec, stride_w, (s->npix + 31) / 32, (int)pairs, (uint32_t*)d_cnt, c->st));
+    CK(c, launch_bitrev(c->L, s->d_bits, stride_w * pairs, c->st));
+    CK(c, launch_bitrev(c->L, s->d_wit, stride_w * pairs, c->st));
     std::vector<uint32_t> h(pairs);
     CK(c, cudaMemcpyAsync(h.data(), d_cnt, 4 * (size_t)pairs, cudaMemcpyDeviceToHost, c->st));
     CK(c, cudaStreamSynchronize(c->st));
@@ -1159,37 +1148,54 @@ extern "C" int rbf_stream_decode_verify(rbf_stream* s, uint32_t pairs, uint64_t*
 // ------------------------------------------------------------------------------------------
 // N1 / N2: changed-value gather and frame reconstruction on the device
 // ------------------------------------------------------------------------------------------
+// byte offsets [pairs + 1] of the encoded pairs' changed values (set pixels x pixel bytes); returns the total
+static uint64_t changed_offsets(const rbf_stream* s, uint32_t pairs, uint64_t* offs) {
+    const uint64_t pb = (uint64_t)s->C * s->S;
+    offs[0] = 0;
+    for (uint32_t i = 0; i < pairs; i++) offs[i + 1] = offs[i] + s->last_infos[i].ones * pb;
+    return offs[pairs];
+}
+
+// The changed values of the encoded pairs [0, pairs) gathered at offs into the values scratch slot, on the context's stream
+// (value_mode 1: residuals against each pair's previous frame).
+static int gather_values(rbf_stream* s, uint32_t pairs, const uint64_t* offs, uint8_t** d_values) {
+    rbf_ctx* c = s->c;
+    const uint32_t pb = s->C * s->S;
+    void *d_vals = nullptr, *d_jobs = nullptr, *d_gcnt = nullptr;
+    int rc;
+    if ((rc = scratch_get(c, kScrValues, (size_t)offs[pairs] + 256, &d_vals)) ||
+        (rc = scratch_get(c, kScrGatherJobs, sizeof(GatherJob) * pairs, &d_jobs)) ||
+        (rc = scratch_get(c, kScrGatherCounts, 4 * (size_t)pairs * gather_chunks((uint32_t)s->npix) + 64, &d_gcnt)))
+        return rc;
+    std::vector<GatherJob> jobs(pairs);
+    for (uint32_t i = 0; i < pairs; i++) {
+        GatherJob& J = jobs[i];
+        J.mask = s->d_mask + (size_t)i * s->mask_stride_w;
+        J.frame = s->h_pairs[i].curr;
+        J.prev = s->h_pairs[i].prev;
+        J.values = (uint8_t*)d_vals + offs[i];
+        J.out_frame = nullptr;
+        J.npix = (uint32_t)s->npix;
+        J.pix_bytes = pb;
+    }
+    CK(c, cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(GatherJob) * pairs, cudaMemcpyHostToDevice, c->st));   // pageable: staged before return
+    CK(c, launch_gather_scatter(c->L, (const GatherJob*)d_jobs, (int)pairs, 0, (uint32_t)s->npix, pb, (uint32_t*)d_gcnt, nullptr, c->st,
+                                s->value_mode ? s->S : 0u));
+    *d_values = (uint8_t*)d_vals;
+    return RBF_OK;
+}
+
 extern "C" int rbf_stream_gather_changed(rbf_stream* s, uint32_t pairs, uint8_t* values_out, uint64_t capacity,
                                          uint64_t* offsets_out) {
     if (!s || !offsets_out) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_gather_changed: NULL");
     rbf_ctx* c = s->c;
     if (pairs == 0 || pairs > s->last_pairs) return set_err(c, RBF_ERR_INVALID, "only %u pairs were encoded", s->last_pairs);
     CK(c, cudaSetDevice(c->device));
-    const uint64_t pb = (uint64_t)s->C * s->S;
-    uint64_t total = 0;
-    for (uint32_t i = 0; i < pairs; i++) { offsets_out[i] = total; total += s->last_infos[i].ones * pb; }
-    offsets_out[pairs] = total;
+    const uint64_t total = changed_offsets(s, pairs, offsets_out);
     if (!values_out) return RBF_OK;                      // size query
     if (capacity < total) return set_err(c, RBF_ERR_INVALID, "values buffer too small: %llu < %llu", (unsigned long long)capacity, (unsigned long long)total);
-    void *d_vals, *d_jobs, *d_gcnt;
-    int rc;
-    if ((rc = scratch_get(c, 8, (size_t)total + 256, &d_vals)) || (rc = scratch_get(c, 9, sizeof(GatherJob) * pairs, &d_jobs)) ||
-        (rc = scratch_get(c, 13, 4 * (size_t)pairs * gather_chunks((uint32_t)s->npix) + 64, &d_gcnt)))
-        return rc;
-    std::vector<GatherJob> jobs(pairs);
-    for (uint32_t i = 0; i < pairs; i++) {
-        jobs[i].mask = s->d_mask + (size_t)i * s->mask_stride_w;
-        jobs[i].frame = s->h_pairs[i].curr;
-        jobs[i].prev = s->h_pairs[i].prev;
-        jobs[i].values = (uint8_t*)d_vals + offsets_out[i];
-        jobs[i].out_frame = nullptr;
-        jobs[i].npix = (uint32_t)s->npix;
-        jobs[i].pix_bytes = (uint32_t)pb;
-    }
-    CK(c, cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(GatherJob) * pairs, cudaMemcpyHostToDevice, c->st));
-    LAUNCH(c, launch_gather_scatter((const GatherJob*)d_jobs, (int)pairs, 0, (uint32_t)s->npix, (uint32_t)pb, (uint32_t*)d_gcnt, nullptr, c->st,
-                                    s->value_mode ? s->S : 0u));
-    c->launches++;
+    uint8_t* d_vals;
+    if (int r = gather_values(s, pairs, offsets_out, &d_vals)) return r;
     if (total) { CK(c, cudaMemcpyAsync(values_out, d_vals, (size_t)total, cudaMemcpyDeviceToHost, c->st)); c->d2h += (int64_t)total; }
     CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
@@ -1205,8 +1211,9 @@ extern "C" int rbf_stream_apply_diff(rbf_stream* s, uint32_t base_frame, uint32_
     const size_t mbytes = (size_t)((s->npix + 7) / 8), mwords = s->mask_stride_w;
     void *d_mask, *d_vals, *d_job, *d_gcnt;
     int rc;
-    if ((rc = scratch_get(c, 10, mwords * 4, &d_mask)) || (rc = scratch_get(c, 8, (size_t)values_bytes + 256, &d_vals)) ||
-        (rc = scratch_get(c, 9, sizeof(GatherJob) + 64, &d_job)) || (rc = scratch_get(c, 13, 4 * (size_t)gather_chunks((uint32_t)s->npix) + 64, &d_gcnt)))
+    if ((rc = scratch_get(c, kScrApplyMask, mwords * 4, &d_mask)) || (rc = scratch_get(c, kScrValues, (size_t)values_bytes + 256, &d_vals)) ||
+        (rc = scratch_get(c, kScrGatherJobs, sizeof(GatherJob) + 64, &d_job)) ||
+        (rc = scratch_get(c, kScrGatherCounts, 4 * (size_t)gather_chunks((uint32_t)s->npix) + 64, &d_gcnt)))
         return rc;
     CK(c, cudaMemsetAsync(d_mask, 0, mwords * 4, c->st));
     CK(c, cudaMemcpyAsync(d_mask, mask_packed_little, mbytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)mbytes;
@@ -1220,15 +1227,14 @@ extern "C" int rbf_stream_apply_diff(rbf_stream* s, uint32_t base_frame, uint32_
     uint32_t* d_cnt = (uint32_t*)((uint8_t*)d_job + sizeof(GatherJob));
     // the reference applies the diff only when the value count matches the mask (ivc:882): count first
     CK(c, cudaMemsetAsync(d_cnt, 0, 4, c->st));
-    LAUNCH(c, launch_popcount((const uint32_t*)d_mask, (s->npix + 31) / 32, d_cnt, c->sm_count, c->st));
+    CK(c, launch_popcount(c->L, (const uint32_t*)d_mask, (s->npix + 31) / 32, d_cnt, c->st));
     uint32_t h_cnt = 0;
     CK(c, cudaMemcpyAsync(&h_cnt, d_cnt, 4, cudaMemcpyDeviceToHost, c->st));
     CK(c, cudaStreamSynchronize(c->st));
     if (applied_pixels) *applied_pixels = 0;
     if ((uint64_t)h_cnt * pb != values_bytes) return RBF_OK;       // ivc:882: mismatch -> the base frame is returned unchanged
     CK(c, cudaMemcpyAsync(d_job, &J, sizeof J, cudaMemcpyHostToDevice, c->st));
-    LAUNCH(c, launch_gather_scatter((const GatherJob*)d_job, 1, 1, (uint32_t)s->npix, (uint32_t)pb, (uint32_t*)d_gcnt, nullptr, c->st));
-    c->launches++;
+    CK(c, launch_gather_scatter(c->L, (const GatherJob*)d_job, 1, 1, (uint32_t)s->npix, (uint32_t)pb, (uint32_t*)d_gcnt, nullptr, c->st));
     CK(c, cudaStreamSynchronize(c->st));
     if (applied_pixels) *applied_pixels = h_cnt;
     return RBF_OK;
@@ -1268,7 +1274,7 @@ extern "C" int rbf_stream_decode_masks(rbf_stream* s, uint32_t count, const uint
     CK(c, cudaSetDevice(c->device));
     if (int r = wait_pack(c)) return r;                  // the bit arrays are overwritten
     void* d_cnt;
-    if (int r = scratch_get(c, 21, 8 * (size_t)count, &d_cnt)) return r;
+    if (int r = scratch_get(c, kScrDecodeCounts, 8 * (size_t)count, &d_cnt)) return r;
     uint32_t* d_consumed = (uint32_t*)d_cnt;
     uint32_t* d_ones = d_consumed + count;
     CK(c, cudaMemcpy2DAsync(s->d_bits, stride, bitmaps, bitmap_slot, bitmap_slot, count, cudaMemcpyHostToDevice, c->st));
@@ -1279,39 +1285,28 @@ extern "C" int rbf_stream_decode_masks(rbf_stream* s, uint32_t count, const uint
     }
     // packbits order -> LSB-first words.  k_bitrev reverses each byte in place, so whatever lies past a slot is only reordered,
     // and nothing reads a bit array at or past bit l or a witness at or past bit wlen
-    LAUNCH(c, launch_bitrev(s->d_bits, s->mask_stride_w * count, c->sm_count, c->st));
-    if (witness_slot) LAUNCH(c, launch_bitrev(s->d_wit, s->mask_stride_w * count, c->sm_count, c->st));
+    CK(c, launch_bitrev(c->L, s->d_bits, s->mask_stride_w * count, c->st));
+    if (witness_slot) CK(c, launch_bitrev(c->L, s->d_wit, s->mask_stride_w * count, c->st));
     CK(c, cudaMemsetAsync(s->d_mask, 0, stride * count, c->st));       // K4b ORs into the mask slots
     CK(c, cudaMemsetAsync(d_cnt, 0, 8 * (size_t)count, c->st));
     const uint32_t ncent = (uint32_t)((n + 99) / 100);
     uint32_t total_cent = 0, max_l = 0, coded = 0;
     s->h_prefix[0] = 0;
     for (uint32_t i = 0; i < count; i++) {
-        FrameJob& J = s->h_jobs[i];
-        memset(&J, 0, sizeof J);
-        J.n = (uint32_t)n;
-        J.bits = s->d_bits + (size_t)i * s->mask_stride_w;
-        J.witness = s->d_wit + (size_t)i * s->mask_stride_w;
-        J.pass = s->d_pass + (size_t)i * s->pass_stride_w;
-        J.out_mask = s->d_mask + (size_t)i * s->mask_stride_w;
-        if (!raw[i]) {                                    // the payload's float64 k (ivc:275-279)
-            job_set_filter(J, l[i], k[i], *sd);
-            J.wlen_in = (uint32_t)wlen[i];
-            total_cent += ncent; coded++;
-            if (l[i] > max_l) max_l = (uint32_t)l[i];
-        }
+        const uint64_t li = raw[i] ? 0 : l[i];                // the payload's float64 k (ivc:275-279)
+        slot_job(s, i, li, k[i], *sd, s->d_mask + (size_t)i * s->mask_stride_w, wlen[i]);
+        if (li) { total_cent += ncent; coded++; }
+        if (li > max_l) max_l = (uint32_t)li;
         s->h_prefix[i + 1] = total_cent;
     }
-    CK(c, cudaMemcpyAsync(s->d_jobs, s->h_jobs, sizeof(FrameJob) * count, cudaMemcpyHostToDevice, c->st));
     if (coded) {
-        CK(c, cudaMemcpyAsync(s->d_prefix, s->h_prefix, 4 * ((size_t)count + 1), cudaMemcpyHostToDevice, c->st));
-        LAUNCH(c, launch_query(s->d_jobs, s->d_prefix, (int)count, total_cent, max_l, c->query_variant, c->sm_count, c->query_smem_cap,
-                               c->query_warps, c->st));
-        LAUNCH(c, launch_expand(s->d_jobs, (int)count, ncent, c->sm_count, s->d_chunkcnt, d_consumed, c->st));
-        c->launches += 1;
+        if (int r = decode_enqueue(c, s->h_jobs, s->d_jobs, s->h_prefix, s->d_prefix, (int)count, max_l, ncent, s->d_chunkcnt, d_consumed))
+            return r;
+    } else {
+        CK(c, cudaMemcpyAsync(s->d_jobs, s->h_jobs, sizeof(FrameJob) * count, cudaMemcpyHostToDevice, c->st));
     }
-    if (coded < count) LAUNCH(c, launch_raw_masks(s->d_jobs, (int)count, (uint32_t)n, c->st));
-    LAUNCH(c, launch_mask_popcount(s->d_mask, s->mask_stride_w, (uint32_t)n, (int)count, d_ones, c->sm_count, c->st));
+    if (coded < count) CK(c, launch_raw_masks(c->L, s->d_jobs, (int)count, (uint32_t)n, c->st));
+    CK(c, launch_mask_popcount(c->L, s->d_mask, s->mask_stride_w, (uint32_t)n, (int)count, d_ones, c->st));
     std::vector<uint32_t> h(2 * (size_t)count);
     CK(c, cudaMemcpyAsync(h.data(), d_cnt, 8 * (size_t)count, cudaMemcpyDeviceToHost, c->st));
     c->d2h += 8 * (int64_t)count;
@@ -1354,8 +1349,8 @@ extern "C" int rbf_stream_apply_chain_modes(rbf_stream* s, uint32_t base_frame, 
     // d_small: the value offsets, then the residual flags (one H2D copy for both), then first_bad and the totals
     const size_t off_bytes = 8 * ((size_t)count + 1), flag_bytes = residual ? count : 0, res_at = align_up(off_bytes + flag_bytes, 16);
     const size_t small = res_at + 4 * ((size_t)count + 1);
-    if ((rc = scratch_get(c, 8, (size_t)vbytes + 256, &d_vals)) || (rc = scratch_get(c, 22, small, &d_small)) ||
-        (rc = scratch_get(c, 23, 4 * (size_t)count * ntiles, &d_pfx)))
+    if ((rc = scratch_get(c, kScrValues, (size_t)vbytes + 256, &d_vals)) || (rc = scratch_get(c, kScrChainSmall, small, &d_small)) ||
+        (rc = scratch_get(c, kScrChainTiles, 4 * (size_t)count * ntiles, &d_pfx)))
         return rc;
     uint64_t* d_off = (uint64_t*)d_small;
     uint32_t* d_res = (uint32_t*)((uint8_t*)d_small + res_at);   // [0] first_bad, [1 + i] totals
@@ -1379,8 +1374,7 @@ extern "C" int rbf_stream_apply_chain_modes(rbf_stream* s, uint32_t base_frame, 
     A.residual = any_residual ? (const uint8_t*)d_small + off_bytes : nullptr;   // a group without residual pairs runs the plain sweep
     A.sample_bytes = s->S;
     A.tile_pfx = (uint32_t*)d_pfx; A.totals = d_res + 1; A.first_bad = d_res;
-    LAUNCH(c, launch_apply_chain(A, c->sm_count, c->st));
-    c->launches += 2;                                   // tile count + tile scan
+    CK(c, launch_apply_chain(c->L, A, c->st));
     std::vector<uint32_t> h((size_t)count + 1);
     CK(c, cudaMemcpyAsync(h.data(), d_res, 4 * ((size_t)count + 1), cudaMemcpyDeviceToHost, c->st));
     c->d2h += 4 * ((int64_t)count + 1);
@@ -1415,9 +1409,9 @@ extern "C" int rbf_median_blur5(rbf_ctx* c, const void* plane_in, uint32_t H, ui
     const size_t bytes = (size_t)H * W * sample_bytes;
     void *d_in, *d_out;
     int rc;
-    if ((rc = scratch_get(c, 11, bytes, &d_in)) || (rc = scratch_get(c, 12, bytes, &d_out))) return rc;
+    if ((rc = scratch_get(c, kScrMedianIn, bytes, &d_in)) || (rc = scratch_get(c, kScrMedianOut, bytes, &d_out))) return rc;
     CK(c, cudaMemcpyAsync(d_in, plane_in, bytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)bytes;
-    LAUNCH(c, launch_median5(d_in, 1, H, W, (int)sample_bytes, d_out, c->st));
+    CK(c, launch_median5(c->L, d_in, 1, H, W, (int)sample_bytes, d_out, c->st));
     CK(c, cudaMemcpyAsync(plane_out, d_out, bytes, cudaMemcpyDeviceToHost, c->st)); c->d2h += (int64_t)bytes;
     CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
@@ -1430,8 +1424,8 @@ extern "C" int rbf_stream_median5(rbf_stream* s, uint32_t frame, void* plane_out
     const size_t bytes = (size_t)s->npix * s->S;
     void* d_out;
     int rc;
-    if ((rc = scratch_get(c, 12, bytes, &d_out))) return rc;
-    LAUNCH(c, launch_median5(s->d_frames + (size_t)frame * s->frame_stride, s->C, s->H, s->W, (int)s->S, d_out, c->st));
+    if ((rc = scratch_get(c, kScrMedianOut, bytes, &d_out))) return rc;
+    CK(c, launch_median5(c->L, s->d_frames + (size_t)frame * s->frame_stride, s->C, s->H, s->W, (int)s->S, d_out, c->st));
     CK(c, cudaMemcpyAsync(plane_out, d_out, bytes, cudaMemcpyDeviceToHost, c->st)); c->d2h += (int64_t)bytes;
     CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
@@ -1462,14 +1456,15 @@ static int zlib_batch(rbf_ctx* c, uint32_t count, const void* const* srcs, const
     if (count == 0) return RBF_OK;
     for (uint32_t b = 0; b < count; b++)
         if (lens[b] && !srcs[b]) return set_err(c, RBF_ERR_INVALID, "zlib: buffer %u is NULL", b);
-    const uint32_t W = 2u * (uint32_t)(c->sm_count > 0 ? c->sm_count : 1);
+    const uint32_t W = 2u * (uint32_t)(c->L.sm_count > 0 ? c->L.sm_count : 1);
     const size_t region = align_up(deflate_seg_bound(kDeflateSeg), 16), stage_cap = (size_t)W * (region + 8);
     void *d_in = nullptr, *d_res, *d_out, *d_stage, *d_segs, *d_copies, *d_small;
     int rc;
-    if ((rc = scratch_get(c, 14, (size_t)W * kDeflateSeg * 4, &d_res)) || (rc = scratch_get(c, 15, (size_t)W * region, &d_out)) ||
-        (rc = scratch_get(c, 16, stage_cap, &d_stage)) || (rc = scratch_get(c, 17, (size_t)W * sizeof(DeflateSeg), &d_segs)) ||
-        (rc = scratch_get(c, 18, (size_t)W * sizeof(DeflateCopy), &d_copies)) || (rc = scratch_get(c, 19, (size_t)W * 12 + 64, &d_small)) ||
-        (!on_device && (rc = scratch_get(c, 20, (size_t)W * kDeflateSeg, &d_in))))
+    if ((rc = scratch_get(c, kScrZlibRes, (size_t)W * kDeflateSeg * 4, &d_res)) || (rc = scratch_get(c, kScrZlibOut, (size_t)W * region, &d_out)) ||
+        (rc = scratch_get(c, kScrZlibStage, stage_cap, &d_stage)) || (rc = scratch_get(c, kScrZlibSegs, (size_t)W * sizeof(DeflateSeg), &d_segs)) ||
+        (rc = scratch_get(c, kScrZlibCopies, (size_t)W * sizeof(DeflateCopy), &d_copies)) ||
+        (rc = scratch_get(c, kScrZlibSmall, (size_t)W * 12 + 64, &d_small)) ||
+        (!on_device && (rc = scratch_get(c, kScrZlibIn, (size_t)W * kDeflateSeg, &d_in))))
         return rc;
     uint32_t* d_sizes = (uint32_t*)d_small;
     uint32_t* d_adler = d_sizes + W;
@@ -1509,7 +1504,7 @@ static int zlib_batch(rbf_ctx* c, uint32_t count, const void* const* srcs, const
         }
         CK(c, cudaMemsetAsync(d_err, 0, 4, c->st));
         CK(c, cudaMemcpyAsync(d_segs, segs.data(), sizeof(DeflateSeg) * n, cudaMemcpyHostToDevice, c->st));
-        LAUNCH(c, launch_deflate_segments((const DeflateSeg*)d_segs, (int)n, (uint32_t*)d_res, d_sizes, d_adler, d_err, c->st));
+        CK(c, launch_deflate_segments(c->L, (const DeflateSeg*)d_segs, (int)n, (uint32_t*)d_res, d_sizes, d_adler, d_err, c->st));
         CK(c, cudaMemcpyAsync(h_small.data(), d_small, (3 * (size_t)W + 1) * 4, cudaMemcpyDeviceToHost, c->st));
         CK(c, cudaStreamSynchronize(c->st));
         if (h_small[3 * (size_t)W]) return set_err(c, RBF_ERR_STATE, "zlib: a coded segment overran its region (flags %u)", h_small[3 * (size_t)W]);
@@ -1535,7 +1530,7 @@ static int zlib_batch(rbf_ctx* c, uint32_t count, const void* const* srcs, const
             return set_err(c, RBF_ERR_INVALID, "zlib: output buffer too small (%llu < %llu so far)", (unsigned long long)capacity,
                            (unsigned long long)pos);
         CK(c, cudaMemcpyAsync(d_copies, copies.data(), sizeof(DeflateCopy) * n, cudaMemcpyHostToDevice, c->st));
-        LAUNCH(c, launch_deflate_concat((const DeflateCopy*)d_copies, (int)n, (uint8_t*)d_stage, stage_cap, d_err, c->st));
+        CK(c, launch_deflate_concat(c->L, (const DeflateCopy*)d_copies, (int)n, (uint8_t*)d_stage, stage_cap, d_err, c->st));
         CK(c, cudaMemcpyAsync(out_host + wave_start, d_stage, (size_t)(pos - wave_start), cudaMemcpyDeviceToHost, c->st));
         CK(c, cudaMemcpyAsync(h_small.data() + 3 * (size_t)W, d_err, 4, cudaMemcpyDeviceToHost, c->st));
         c->d2h += (int64_t)(pos - wave_start);
@@ -1556,34 +1551,13 @@ extern "C" int rbf_stream_zlib_changed(rbf_stream* s, uint32_t pairs, uint8_t* o
     rbf_ctx* c = s->c;
     if (pairs == 0 || pairs > s->last_pairs) return set_err(c, RBF_ERR_INVALID, "only %u pairs were encoded", s->last_pairs);
     CK(c, cudaSetDevice(c->device));
-    const uint64_t pb = (uint64_t)s->C * s->S;
     std::vector<uint64_t> voff(pairs + 1);
-    uint64_t total = 0;
-    for (uint32_t i = 0; i < pairs; i++) { voff[i] = total; total += s->last_infos[i].ones * pb; }
-    voff[pairs] = total;
-    void *d_vals, *d_jobs, *d_gcnt;
-    int rc;
-    if ((rc = scratch_get(c, 8, (size_t)total + 256, &d_vals)) || (rc = scratch_get(c, 9, sizeof(GatherJob) * pairs, &d_jobs)) ||
-        (rc = scratch_get(c, 13, 4 * (size_t)pairs * gather_chunks((uint32_t)s->npix) + 64, &d_gcnt)))
-        return rc;
-    std::vector<GatherJob> jobs(pairs);
+    changed_offsets(s, pairs, voff.data());
+    uint8_t* d_vals;
+    if (int r = gather_values(s, pairs, voff.data(), &d_vals)) return r;
     std::vector<const void*> srcs(pairs);
     std::vector<uint64_t> lens(pairs);
-    for (uint32_t i = 0; i < pairs; i++) {
-        jobs[i].mask = s->d_mask + (size_t)i * s->mask_stride_w;
-        jobs[i].frame = s->h_pairs[i].curr;
-        jobs[i].prev = s->h_pairs[i].prev;
-        jobs[i].values = (uint8_t*)d_vals + voff[i];
-        jobs[i].out_frame = nullptr;
-        jobs[i].npix = (uint32_t)s->npix;
-        jobs[i].pix_bytes = (uint32_t)pb;
-        srcs[i] = jobs[i].values;
-        lens[i] = voff[i + 1] - voff[i];
-    }
-    CK(c, cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(GatherJob) * pairs, cudaMemcpyHostToDevice, c->st));
-    LAUNCH(c, launch_gather_scatter((const GatherJob*)d_jobs, (int)pairs, 0, (uint32_t)s->npix, (uint32_t)pb, (uint32_t*)d_gcnt, nullptr, c->st,
-                                    s->value_mode ? s->S : 0u));
-    c->launches++;
+    for (uint32_t i = 0; i < pairs; i++) { srcs[i] = d_vals + voff[i]; lens[i] = voff[i + 1] - voff[i]; }
     return zlib_batch(c, pairs, srcs.data(), lens.data(), true, out_host, out_capacity, out_offsets);   // same stream: after the gather
 }
 
@@ -1643,7 +1617,7 @@ static int nccl_allgather_on(rbf_ctx* c, const void* d_send, void* d_recv, uint6
         fn_GetErrorString es = (fn_GetErrorString)dlsym(c->nccl_lib, "ncclGetErrorString");
         return set_err(c, RBF_ERR_NCCL, "ncclAllGather failed: %s", es ? es(r) : "?");
     }
-    c->launches++;
+    c->L.launches++;
     return RBF_OK;
 }
 extern "C" int rbf_nccl_allgather(rbf_ctx* c, const void* d_send, void* d_recv, uint64_t bytes_per_rank) {
@@ -1675,14 +1649,13 @@ extern "C" int rbf_stream_allgather_bitmaps(rbf_stream* s, uint32_t pairs, uint6
         CK(c, cudaStreamWaitEvent(c->st_comm, c->ev_enc, 0));
         // every rank has signalled the previous exchange => it has consumed the one before it: that half is free everywhere
         if (c->peer_seq > 0)
-            LAUNCH(c, launch_peer_wait(c->peer_flags[c->peer_rank], c->peer_nranks, c->peer_seq, kPeerTimeoutCycles, c->peer_err, c->st_comm));
+            CK(c, launch_peer_wait(c->L, c->peer_flags[c->peer_rank], c->peer_nranks, c->peer_seq, kPeerTimeoutCycles, c->peer_err, c->st_comm));
         c->peer_seq++;
         const uint32_t slot_w = (uint32_t)(slot_bytes / 4);
         const size_t half_w = (size_t)c->peer_nranks * pairs * slot_w;
         const size_t dst_off_w = (size_t)(c->peer_seq & 1u) * half_w + (size_t)c->peer_rank * pairs * slot_w;
-        LAUNCH(c, launch_push_slots(s->d_bits, s->mask_stride_w, slot_w, pairs, c->peer_recv, c->peer_flags, c->peer_nranks, c->peer_rank,
-                                    dst_off_w, c->peer_seq, c->sm_count, c->st_comm));
-        c->launches++;                                              // push + signal
+        CK(c, launch_push_slots(c->L, s->d_bits, s->mask_stride_w, slot_w, pairs, c->peer_recv, c->peer_flags, c->peer_nranks, c->peer_rank,
+                                    dst_off_w, c->peer_seq, c->st_comm));
         CK(c, cudaEventRecord(c->ev_pack, c->st_comm));
         CK(c, cudaEventRecord(c->ev_comm, c->st_comm));
         c->pack_pending = c->comm_pending = c->peer_wait_pending = true;

@@ -114,10 +114,16 @@ __device__ __forceinline__ void or_bits128(uint32_t* __restrict__ W, uint64_t bi
 // ------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------
+// the launch status of the `kernels` kernels just enqueued, which are added to the context's counter
+static cudaError_t counted(LaunchCfg& L, int kernels = 1) {
+    L.launches += kernels;
+    return cudaGetLastError();
+}
+
 // K1 over a chain of F >= 2 pairs: persistent CTAs, at most ctas_per_sm per SM, each sweeping the same number of tiles (or one fewer)
 template <int PB, int S, bool GRAY>
-static cudaError_t launch_threshold_sweep_t(const PairJob* d_pairs, int F, uint32_t npix, int thr, int any_mode, uint32_t* d_ones,
-                                            uint32_t* d_resid, int sm_count, int ctas_per_sm, cudaStream_t st) {
+static cudaError_t launch_threshold_sweep_t(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t npix, int thr, int any_mode,
+                                            uint32_t* d_ones, uint32_t* d_resid, int ctas_per_sm, cudaStream_t st) {
     const int smem = SW_STAGES * (int)SW_TILE_PX * PB;
     cudaError_t e = cudaFuncSetAttribute(k_threshold_sweep<PB, S, GRAY>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return e;
@@ -128,78 +134,65 @@ static cudaError_t launch_threshold_sweep_t(const PairJob* d_pairs, int F, uint3
     if (per_sm > cap) per_sm = cap;
     if (per_sm < 1) per_sm = 1;
     const uint32_t ntiles = (npix + SW_TILE_PX - 1u) / SW_TILE_PX;
-    const uint32_t slots = (uint32_t)(sm_count > 0 ? sm_count : 1) * (uint32_t)per_sm;
+    const uint32_t slots = (uint32_t)(L.sm_count > 0 ? L.sm_count : 1) * (uint32_t)per_sm;
     const uint32_t rounds = (ntiles + slots - 1u) / slots;
     const uint32_t grid = (ntiles + rounds - 1u) / rounds;
     k_threshold_sweep<PB, S, GRAY><<<grid, SW_THREADS, smem, st>>>(d_pairs, (uint32_t)F, npix, thr, any_mode, d_ones, d_resid);
-    return cudaGetLastError();
+    return counted(L);
 }
 
-template <int PB, int S>
-static cudaError_t launch_threshold_t(const PairJob* d_pairs, int F, uint32_t npix, int thr, int any_mode, uint32_t* d_ones,
-                                      uint32_t* d_resid, int variant, bool chain, int sm_count, int ctas_per_sm, cudaStream_t st) {
+// GRAY: the mask is taken on cv2.COLOR_BGR2GRAY of the three samples instead of on sample 0 (ivc:792-795); no TMA kernel for it
+template <int PB, int S, bool GRAY>
+static cudaError_t launch_threshold_t(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t npix, int thr, int any_mode, uint32_t* d_ones,
+                                      uint32_t* d_resid, bool chain, int ctas_per_sm, cudaStream_t st) {
     const uint32_t nwords = (npix + 31u) >> 5;
     constexpr uint32_t TP = TMA_TILE_BYTES / PB;
-    if (variant == 1 && npix >= TP && (TP / 32u / (TMA_THREADS / 32)) <= 32u) {
-        const int smem = 2 * TMA_STAGES * TMA_TILE_BYTES;
-        cudaError_t e = cudaFuncSetAttribute(k_threshold_tma<PB, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return e;
-        const uint64_t total = (uint64_t)(npix / TP) * (uint64_t)F;
-        int grid = (int)((total < (uint64_t)(2 * sm_count)) ? total : (uint64_t)(2 * sm_count));
-        k_threshold_tma<PB, S><<<grid, TMA_THREADS, smem, st>>>(d_pairs, F, npix, thr, any_mode, d_ones, d_resid);
-        e = cudaGetLastError();
-        if (e != cudaSuccess) return e;
-        const uint32_t px_begin = (npix / TP) * TP;
-        if (px_begin < npix) {
-            const uint32_t tail_words = nwords - (px_begin >> 5);
-            dim3 g((tail_words + 255u) / 256u, (unsigned)F);
-            k_threshold_tail<PB, S><<<g, 256, 0, st>>>(d_pairs, npix, px_begin, thr, any_mode, d_ones, d_resid);
+    if constexpr (!GRAY) {
+        if (L.k1_variant == 1 && npix >= TP && (TP / 32u / (TMA_THREADS / 32)) <= 32u) {
+            const int smem = 2 * TMA_STAGES * TMA_TILE_BYTES;
+            cudaError_t e = cudaFuncSetAttribute(k_threshold_tma<PB, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+            if (e != cudaSuccess) return e;
+            const uint64_t total = (uint64_t)(npix / TP) * (uint64_t)F;
+            int grid = (int)((total < (uint64_t)(2 * L.sm_count)) ? total : (uint64_t)(2 * L.sm_count));
+            k_threshold_tma<PB, S><<<grid, TMA_THREADS, smem, st>>>(d_pairs, F, npix, thr, any_mode, d_ones, d_resid);
+            e = counted(L);
+            if (e != cudaSuccess) return e;
+            const uint32_t px_begin = (npix / TP) * TP;
+            if (px_begin < npix) {
+                const uint32_t tail_words = nwords - (px_begin >> 5);
+                dim3 g((tail_words + 255u) / 256u, (unsigned)F);
+                k_threshold_tail<PB, S><<<g, 256, 0, st>>>(d_pairs, npix, px_begin, thr, any_mode, d_ones, d_resid);
+                return counted(L);
+            }
+            return cudaSuccess;
         }
-        return cudaGetLastError();
     }
-    if (chain && F >= 2) return launch_threshold_sweep_t<PB, S, false>(d_pairs, F, npix, thr, any_mode, d_ones, d_resid, sm_count, ctas_per_sm, st);
+    if (chain && F >= 2) return launch_threshold_sweep_t<PB, S, GRAY>(L, d_pairs, F, npix, thr, any_mode, d_ones, d_resid, ctas_per_sm, st);
     uint32_t bx = (nwords + 255u) / 256u;
-    const uint32_t cap = (uint32_t)(sm_count * (ctas_per_sm > 0 ? ctas_per_sm : 32));
+    const uint32_t cap = (uint32_t)(L.sm_count * (ctas_per_sm > 0 ? ctas_per_sm : 32));
     if ((uint64_t)bx * (uint64_t)F > cap) { bx = (cap + (uint32_t)F - 1u) / (uint32_t)F; if (bx < 1u) bx = 1u; }
     dim3 grid(bx, (unsigned)F);
     const int smem = K1_STAGE_BYTES_PER_PB * PB;
-    cudaError_t e = cudaFuncSetAttribute(k_threshold<PB, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(k_threshold<PB, S, GRAY>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return e;
-    k_threshold<PB, S><<<grid, K1_THREADS, smem, st>>>(d_pairs, npix, thr, any_mode, d_ones, d_resid);
-    return cudaGetLastError();
+    k_threshold<PB, S, GRAY><<<grid, K1_THREADS, smem, st>>>(d_pairs, npix, thr, any_mode, d_ones, d_resid);
+    return counted(L);
 }
 
-// gray_mode: the mask is taken on cv2.COLOR_BGR2GRAY of the three samples instead of on sample 0 (ivc:792-795)
-template <int PB, int S>
-static cudaError_t launch_threshold_gray_t(const PairJob* d_pairs, int F, uint32_t npix, int thr, int any_mode, uint32_t* d_ones,
-                                           uint32_t* d_resid, bool chain, int sm_count, int ctas_per_sm, cudaStream_t st) {
-    if (chain && F >= 2) return launch_threshold_sweep_t<PB, S, true>(d_pairs, F, npix, thr, any_mode, d_ones, d_resid, sm_count, ctas_per_sm, st);
-    const uint32_t nwords = (npix + 31u) >> 5;
-    uint32_t bx = (nwords + 255u) / 256u;
-    const uint32_t cap = (uint32_t)(sm_count * (ctas_per_sm > 0 ? ctas_per_sm : 32));
-    if ((uint64_t)bx * (uint64_t)F > cap) { bx = (cap + (uint32_t)F - 1u) / (uint32_t)F; if (bx < 1u) bx = 1u; }
-    dim3 grid(bx, (unsigned)F);
-    const int smem = K1_STAGE_BYTES_PER_PB * PB;
-    cudaError_t e = cudaFuncSetAttribute(k_threshold<PB, S, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    k_threshold<PB, S, true><<<grid, K1_THREADS, smem, st>>>(d_pairs, npix, thr, any_mode, d_ones, d_resid);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_threshold(const PairJob* d_pairs, int F, uint32_t npix, int channels, int sample_bytes, int thr_int,
-                             int any_mode, int gray_mode, uint32_t* d_ones, uint32_t* d_resid, int variant, bool chain,
-                             int sm_count, int ctas_per_sm, cudaStream_t st) {
+cudaError_t launch_threshold(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t npix, int channels, int sample_bytes, int thr_int,
+                             int any_mode, int gray_mode, uint32_t* d_ones, uint32_t* d_resid, bool chain, bool pipelined,
+                             cudaStream_t st) {
     if (F <= 0 || npix == 0) return cudaSuccess;
-    const int pb = channels * sample_bytes;
+    const int pb = channels * sample_bytes, cap = pipelined ? L.pipe_k1_ctas_per_sm : L.k1_ctas_per_sm;
     if (gray_mode) {
-        if (pb == 3 && sample_bytes == 1) return launch_threshold_gray_t<3, 1>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, sm_count, ctas_per_sm, st);
-        if (pb == 6 && sample_bytes == 2) return launch_threshold_gray_t<6, 2>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, sm_count, ctas_per_sm, st);
+        if (pb == 3 && sample_bytes == 1) return launch_threshold_t<3, 1, true>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, st);
+        if (pb == 6 && sample_bytes == 2) return launch_threshold_t<6, 2, true>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, st);
         return cudaErrorInvalidValue;
     }
-    if (pb == 3 && sample_bytes == 1) return launch_threshold_t<3, 1>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, variant, chain, sm_count, ctas_per_sm, st);
-    if (pb == 6 && sample_bytes == 2) return launch_threshold_t<6, 2>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, variant, chain, sm_count, ctas_per_sm, st);
-    if (pb == 1 && sample_bytes == 1) return launch_threshold_t<1, 1>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, variant, chain, sm_count, ctas_per_sm, st);
-    if (pb == 2 && sample_bytes == 2) return launch_threshold_t<2, 2>(d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, variant, chain, sm_count, ctas_per_sm, st);
+    if (pb == 3 && sample_bytes == 1) return launch_threshold_t<3, 1, false>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, st);
+    if (pb == 6 && sample_bytes == 2) return launch_threshold_t<6, 2, false>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, st);
+    if (pb == 1 && sample_bytes == 1) return launch_threshold_t<1, 1, false>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, st);
+    if (pb == 2 && sample_bytes == 2) return launch_threshold_t<2, 2, false>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, st);
     return cudaErrorInvalidValue;
 }
 
@@ -225,28 +218,27 @@ static cudaError_t insert_cluster_occupancy(uint32_t cs, int* clusters) {
     return cudaOccupancyMaxActiveClusters(clusters, k_insert_cluster, &cfg);
 }
 
-cudaError_t launch_insert(const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t max_l_bits, int variant, int sm_count,
-                          int* k2_clusters, cudaStream_t st) {
+cudaError_t launch_insert(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t max_l_bits, cudaStream_t st) {
     if (F <= 0 || max_centuries == 0) return cudaSuccess;
     const uint32_t words = (uint32_t)(((uint64_t)max_l_bits + 31u) >> 5);
-    if (variant >= 1 && words > 2u * K2_MAX_CS * K2_WORDS) {   // less than half of the array would be on chip: RED.OR into L2
+    if (L.insert_variant >= 1 && words > 2u * K2_MAX_CS * K2_WORDS) {   // less than half of the array would be on chip: RED.OR into L2
         const uint32_t nslab = (max_centuries + 31u) / 32u;
         dim3 grid((nslab + I2_WARPS - 1) / I2_WARPS, (unsigned)F);
         k_insert2<<<grid, I2_WARPS * 32, 0, st>>>(d_jobs);
-        return cudaGetLastError();
+        return counted(L);
     }
-    if (variant >= 1) {                                   // dense, warp-compacted insert into (cluster) shared memory
+    if (L.insert_variant >= 1) {                          // dense, warp-compacted insert into (cluster) shared memory
         uint32_t cs = (words + K2_WORDS - 1u) / K2_WORDS;
         if (cs < 1u) cs = 1u;
         if (cs > (uint32_t)K2_MAX_CS) cs = K2_MAX_CS;    // the rest of the array is set with RED.OR in L2
         // Full waves of resident clusters take one frame each; the frames of the last, partial wave (all of them when F is small)
         // get R copies each so that they still fill the GPU, with at least K2_WARPS slabs per CTA.
-        if (k2_clusters[cs] == 0) {                       // first launch of this shape: measure it once, and refuse it if it does not fit
-            cudaError_t e = insert_cluster_occupancy(cs, &k2_clusters[cs]);
+        if (L.k2_clusters[cs] == 0) {                       // first launch of this shape: measure it once, and refuse it if it does not fit
+            cudaError_t e = insert_cluster_occupancy(cs, &L.k2_clusters[cs]);
             if (e != cudaSuccess) return e;
-            if (k2_clusters[cs] < 1) { k2_clusters[cs] = 0; return cudaErrorInvalidConfiguration; }
+            if (L.k2_clusters[cs] < 1) { L.k2_clusters[cs] = 0; return cudaErrorInvalidConfiguration; }
         }
-        const uint32_t slots = (uint32_t)k2_clusters[cs], full = (uint32_t)F / slots * slots, rem = (uint32_t)F - full;
+        const uint32_t slots = (uint32_t)L.k2_clusters[cs], full = (uint32_t)F / slots * slots, rem = (uint32_t)F - full;
         const uint32_t nslab = (max_centuries + 31u) / 32u;
         const uint32_t useful = (nslab + cs * K2_WARPS - 1u) / (cs * K2_WARPS);
         uint32_t copies = rem ? slots / rem : 1u;
@@ -254,40 +246,42 @@ cudaError_t launch_insert(const FrameJob* d_jobs, int F, uint32_t max_centuries,
         if (copies < 1u) copies = 1u;
         cudaLaunchAttribute attr;
         const cudaLaunchConfig_t cfg = insert_cluster_config(cs, full + rem * copies, st, &attr);
-        return cudaLaunchKernelEx(&cfg, k_insert_cluster, d_jobs, full, copies);
+        const cudaError_t e = cudaLaunchKernelEx(&cfg, k_insert_cluster, d_jobs, full, copies);
+        return e != cudaSuccess ? e : counted(L);
     }
     uint32_t bx = (max_centuries + 255u) / 256u;
-    const uint32_t cap = (uint32_t)(sm_count * 16);
+    const uint32_t cap = (uint32_t)(L.sm_count * 16);
     if ((uint64_t)bx * (uint64_t)F > cap) { bx = (cap + (uint32_t)F - 1u) / (uint32_t)F; if (bx < 1u) bx = 1u; }
     dim3 grid(bx, (unsigned)F);
     k_insert<<<grid, 256, 0, st>>>(d_jobs);
-    return cudaGetLastError();
+    return counted(L);
 }
 
 
 int query_max_smem_bytes() { return 232448 - 1024; }    // 227 KB opt-in minus static shared memory + slack
 
 template <bool HYBRID>
-static cudaError_t launch_query2_t(const FrameJob* d_jobs, const uint32_t* d_cent_prefix, int F, uint32_t total_centuries,
-                                   int sm_count, int smem, cudaStream_t st) {
+static cudaError_t launch_query2_t(LaunchCfg& L, const FrameJob* d_jobs, const uint32_t* d_cent_prefix, int F, uint32_t total_centuries,
+                                   int smem, cudaStream_t st) {
     cudaError_t e = cudaFuncSetAttribute(k_query2<HYBRID>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return e;
-    uint32_t grid = (uint32_t)sm_count;
+    uint32_t grid = (uint32_t)L.sm_count;
     const uint32_t max_useful = (total_centuries + Q2_THREADS - 1) / Q2_THREADS;
     if (grid > max_useful) grid = max_useful;
     if (grid < 1u) grid = 1u;
     k_query2<HYBRID><<<grid, Q2_THREADS, smem, st>>>(d_jobs, d_cent_prefix, F, (uint32_t)((smem - Q2_WARPS * Q2_WARP_WORDS * 4) / 4));
-    return cudaGetLastError();
+    return counted(L);
 }
 
 // variant: 0 per-lane kernel; 1 staged rings; 5 decade tiles (half-decade tiles for 2^23 < m <= 2^24, rings beyond); 6 half-decade
 // tiles for every m <= 2^24.  (2, 3 and 4 selected earlier kernels that were measured slower and removed; the values still
 // select the current default.)
-cudaError_t launch_query(const FrameJob* d_jobs, const uint32_t* d_cent_prefix, int F, uint32_t total_centuries,
-                         uint32_t max_l_bits, int variant, int sm_count, int smem_bytes_cap, int tile_warps, cudaStream_t st) {
+cudaError_t launch_query(LaunchCfg& L, const FrameJob* d_jobs, const uint32_t* d_cent_prefix, int F, uint32_t total_centuries,
+                         uint32_t max_l_bits, cudaStream_t st) {
     if (F <= 0 || total_centuries == 0) return cudaSuccess;
+    int variant = L.query_variant, tile_warps = L.query_warps;
     if (tile_warps < 4 || tile_warps > Q4_WARPS) tile_warps = Q4_WARPS;
-    int cap = smem_bytes_cap & ~15;
+    int cap = L.query_smem_cap & ~15;
     if (cap > query_max_smem_bytes()) cap = query_max_smem_bytes() & ~15;
     const uint32_t need_words = (((max_l_bits + 31u) >> 5) + 3u) & ~3u;
     if (variant >= 2 && variant <= 4) variant = 5;
@@ -298,7 +292,7 @@ cudaError_t launch_query(const FrameJob* d_jobs, const uint32_t* d_cent_prefix, 
         const int bits_cap = cap - qbytes;
         const bool fits = (size_t)need_words * 4 <= (size_t)bits_cap;
         const int smem = qbytes + (fits ? (int)(need_words * 4 < 16 ? 16 : need_words * 4) : bits_cap);
-        uint32_t grid = (uint32_t)sm_count;
+        uint32_t grid = (uint32_t)L.sm_count;
         const uint32_t max_useful = (total_centuries + 32u * tile_warps - 1) / (32u * tile_warps);
         if (grid > max_useful) grid = max_useful;
         if (grid < 1u) grid = 1u;
@@ -312,7 +306,7 @@ cudaError_t launch_query(const FrameJob* d_jobs, const uint32_t* d_cent_prefix, 
         if (fits) { if (half) RBF_LAUNCH_Q4(0, 5); else RBF_LAUNCH_Q4(0, 10); }
         else      { if (half) RBF_LAUNCH_Q4(1, 5); else RBF_LAUNCH_Q4(1, 10); }
 #undef RBF_LAUNCH_Q4
-        return cudaGetLastError();
+        return counted(L);
     }
     if (variant >= 1) {                                   // staged rings (also the home of filters beyond 2^24 bits)
         const int qbytes = Q2_WARPS * Q2_WARP_WORDS * 4;
@@ -320,8 +314,8 @@ cudaError_t launch_query(const FrameJob* d_jobs, const uint32_t* d_cent_prefix, 
         const int bits_cap = cap - qbytes;
         const bool fits = (size_t)need_words * 4 <= (size_t)bits_cap;
         const int smem = qbytes + (fits ? (int)(need_words * 4 < 16 ? 16 : need_words * 4) : bits_cap);
-        return !fits ? launch_query2_t<true>(d_jobs, d_cent_prefix, F, total_centuries, sm_count, smem, st)
-                     : launch_query2_t<false>(d_jobs, d_cent_prefix, F, total_centuries, sm_count, smem, st);
+        return !fits ? launch_query2_t<true>(L, d_jobs, d_cent_prefix, F, total_centuries, smem, st)
+                     : launch_query2_t<false>(L, d_jobs, d_cent_prefix, F, total_centuries, smem, st);
     }
     int smem = (size_t)need_words * 4 > (size_t)cap ? cap : (int)(need_words * 4);
     if (smem < 16) smem = 16;
@@ -331,12 +325,12 @@ cudaError_t launch_query(const FrameJob* d_jobs, const uint32_t* d_cent_prefix, 
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_query, QT, (size_t)smem);
     if (e != cudaSuccess) return e;
     if (per_sm < 1) per_sm = 1;
-    uint32_t grid = (uint32_t)(sm_count * per_sm);
+    uint32_t grid = (uint32_t)(L.sm_count * per_sm);
     const uint32_t max_useful = (total_centuries + QT - 1) / QT;
     if (grid > max_useful) grid = max_useful;
     if (grid < 1u) grid = 1u;
     k_query<<<grid, QT, smem, st>>>(d_jobs, d_cent_prefix, F, (uint32_t)(smem / 4));
-    return cudaGetLastError();
+    return counted(L);
 }
 
 static uint32_t witness_chunks(int F, uint32_t max_centuries, int sm_count) {
@@ -349,22 +343,22 @@ static uint32_t witness_chunks(int F, uint32_t max_centuries, int sm_count) {
     return ch;
 }
 // K3b: d_scratch holds F*32 uint32 (pass counts per chunk)
-cudaError_t launch_witness(const FrameJob* d_jobs, int F, uint32_t max_centuries, int sm_count, uint32_t* d_scratch, uint32_t* d_wlen,
+cudaError_t launch_witness(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t* d_scratch, uint32_t* d_wlen,
                            cudaStream_t st) {
     if (F <= 0) return cudaSuccess;
-    const uint32_t ch = witness_chunks(F, max_centuries, sm_count);
+    const uint32_t ch = witness_chunks(F, max_centuries, L.sm_count);
     if (ch > 1u) k_pass_count<<<dim3(ch, (unsigned)F), 256, 0, st>>>(d_jobs, ch, d_scratch);
     k_witness<<<dim3(ch, (unsigned)F), 1024, 0, st>>>(d_jobs, ch, d_scratch, d_wlen);
     k_finalize<<<dim3(32, (unsigned)F), 256, 0, st>>>(d_jobs, d_wlen);
-    return cudaGetLastError();
+    return counted(L, ch > 1u ? 3 : 2);
 }
-cudaError_t launch_expand(const FrameJob* d_jobs, int F, uint32_t max_centuries, int sm_count, uint32_t* d_scratch, uint32_t* d_consumed,
+cudaError_t launch_expand(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t* d_scratch, uint32_t* d_consumed,
                           cudaStream_t st) {
     if (F <= 0) return cudaSuccess;
-    const uint32_t ch = witness_chunks(F, max_centuries, sm_count);
+    const uint32_t ch = witness_chunks(F, max_centuries, L.sm_count);
     if (ch > 1u) k_pass_count<<<dim3(ch, (unsigned)F), 256, 0, st>>>(d_jobs, ch, d_scratch);
     k_expand<<<dim3(ch, (unsigned)F), 1024, 0, st>>>(d_jobs, ch, d_scratch, d_consumed);
-    return cudaGetLastError();
+    return counted(L, ch > 1u ? 2 : 1);
 }
 static inline unsigned grid_for(size_t n, unsigned block, int sm_count) {
     size_t g = (n + block - 1) / block;
@@ -379,8 +373,8 @@ uint32_t gather_chunks(uint32_t npix) {
     return ch < 1u ? 1u : ch;
 }
 // d_counts: F * gather_chunks(npix) uint32 of scratch; d_totals (may be NULL): set pixels per pair
-cudaError_t launch_gather_scatter(const GatherJob* d_jobs, int F, int scatter, uint32_t npix, uint32_t pix_bytes, uint32_t* d_counts,
-                                  uint32_t* d_totals, cudaStream_t st, uint32_t resid_sample_bytes) {
+cudaError_t launch_gather_scatter(LaunchCfg& L, const GatherJob* d_jobs, int F, int scatter, uint32_t npix, uint32_t pix_bytes,
+                                  uint32_t* d_counts, uint32_t* d_totals, cudaStream_t st, uint32_t resid_sample_bytes) {
     if (F <= 0) return cudaSuccess;
     // the kernel is picked by (pixel bytes, residual sample bytes): 2 B per pixel is one 16-bit sample, never two 8-bit ones
     const uint32_t key = pix_bytes * 4u + resid_sample_bytes;
@@ -400,36 +394,36 @@ cudaError_t launch_gather_scatter(const GatherJob* d_jobs, int F, int scatter, u
     case 6u * 4 + 2: k_gather_scatter<6, 2><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;   // 3 x 16 bit
     default: return cudaErrorInvalidValue;
     }
-    return cudaGetLastError();
+    return counted(L, 2);
 }
-cudaError_t launch_raw_masks(const FrameJob* d_jobs, int F, uint32_t npix, cudaStream_t st) {
+cudaError_t launch_raw_masks(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t npix, cudaStream_t st) {
     if (F <= 0 || npix == 0) return cudaSuccess;
     unsigned gx = (((npix + 31u) >> 5) + 255u) / 256u;
     if (gx > 64u) gx = 64u;
     k_raw_masks<<<dim3(gx, (unsigned)F), 256, 0, st>>>(d_jobs);
-    return cudaGetLastError();
+    return counted(L);
 }
-cudaError_t launch_mask_popcount(const uint32_t* d_masks, size_t stride_w, uint32_t npix, int F, uint32_t* d_out, int sm_count,
+cudaError_t launch_mask_popcount(LaunchCfg& L, const uint32_t* d_masks, size_t stride_w, uint32_t npix, int F, uint32_t* d_out,
                                  cudaStream_t st) {
     if (F <= 0 || npix == 0) return cudaSuccess;
     const uint32_t nwords = (npix + 31u) >> 5;
-    unsigned gx = grid_for(nwords, 256, sm_count);
+    unsigned gx = grid_for(nwords, 256, L.sm_count);
     if (gx > 64u) gx = 64u;
     k_mask_popcount<<<dim3(gx, (unsigned)F), 256, 0, st>>>(d_masks, stride_w, nwords, d_out);
-    return cudaGetLastError();
+    return counted(L);
 }
 template <int PB, int RS>
-static cudaError_t launch_apply_sweep_t(const ApplyChain& A, int sm_count, cudaStream_t st) {
+static cudaError_t launch_apply_sweep_t(LaunchCfg& L, const ApplyChain& A, cudaStream_t st) {
     int per_sm = 1;
     cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_apply_sweep<PB, RS>, AP_THREADS, 0);
     if (e != cudaSuccess) return e;
     if (per_sm < 1) per_sm = 1;
-    const uint32_t slots = (uint32_t)(sm_count > 0 ? sm_count : 1) * (uint32_t)per_sm;
+    const uint32_t slots = (uint32_t)(L.sm_count > 0 ? L.sm_count : 1) * (uint32_t)per_sm;
     const uint32_t rounds = (A.ntiles + slots - 1u) / slots;          // every CTA sweeps the same number of tiles, or one fewer
     k_apply_sweep<PB, RS><<<(A.ntiles + rounds - 1u) / rounds, AP_THREADS, 0, st>>>(A);
-    return cudaGetLastError();
+    return counted(L);
 }
-cudaError_t launch_apply_chain(const ApplyChain& A, int sm_count, cudaStream_t st) {
+cudaError_t launch_apply_chain(LaunchCfg& L, const ApplyChain& A, cudaStream_t st) {
     if (A.count == 0 || A.ntiles == 0) return cudaSuccess;
     // (pixel bytes, residual sample bytes) as in launch_gather_scatter; 0: no residual pair, the plain sweep
     const uint32_t key = A.pix_bytes * 4u + (A.residual ? A.sample_bytes : 0u);
@@ -438,111 +432,116 @@ cudaError_t launch_apply_chain(const ApplyChain& A, int sm_count, cudaStream_t s
         return cudaErrorInvalidValue;
     k_tile_count<<<dim3((A.ntiles + 7u) / 8u, A.count), 256, 0, st>>>(A);
     k_tile_scan<<<A.count, 1024, 0, st>>>(A);
+    L.launches += 2;
     switch (key) {
-    case 1u * 4: return launch_apply_sweep_t<1, 0>(A, sm_count, st);
-    case 2u * 4: return launch_apply_sweep_t<2, 0>(A, sm_count, st);
-    case 3u * 4: return launch_apply_sweep_t<3, 0>(A, sm_count, st);
-    case 6u * 4: return launch_apply_sweep_t<6, 0>(A, sm_count, st);
-    case 1u * 4 + 1: return launch_apply_sweep_t<1, 1>(A, sm_count, st);
-    case 3u * 4 + 1: return launch_apply_sweep_t<3, 1>(A, sm_count, st);
-    case 2u * 4 + 2: return launch_apply_sweep_t<2, 2>(A, sm_count, st);
-    default: return launch_apply_sweep_t<6, 2>(A, sm_count, st);
+    case 1u * 4: return launch_apply_sweep_t<1, 0>(L, A, st);
+    case 2u * 4: return launch_apply_sweep_t<2, 0>(L, A, st);
+    case 3u * 4: return launch_apply_sweep_t<3, 0>(L, A, st);
+    case 6u * 4: return launch_apply_sweep_t<6, 0>(L, A, st);
+    case 1u * 4 + 1: return launch_apply_sweep_t<1, 1>(L, A, st);
+    case 3u * 4 + 1: return launch_apply_sweep_t<3, 1>(L, A, st);
+    case 2u * 4 + 2: return launch_apply_sweep_t<2, 2>(L, A, st);
+    default: return launch_apply_sweep_t<6, 2>(L, A, st);
     }
 }
-cudaError_t launch_median5(const void* d_in, uint32_t pix_stride, uint32_t H, uint32_t W, int sample_bytes, void* d_out, cudaStream_t st) {
+cudaError_t launch_median5(LaunchCfg& L, const void* d_in, uint32_t pix_stride, uint32_t H, uint32_t W, int sample_bytes, void* d_out,
+                           cudaStream_t st) {
     if (H == 0 || W == 0) return cudaSuccess;
     dim3 grid((W + 31u) / 32u, (H + 7u) / 8u);
     if (sample_bytes == 1) k_median5<uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)d_in, pix_stride, H, W, (uint8_t*)d_out);
     else if (sample_bytes == 2) k_median5<uint16_t><<<grid, 256, 0, st>>>((const uint16_t*)d_in, pix_stride, H, W, (uint16_t*)d_out);
     else return cudaErrorInvalidValue;
-    return cudaGetLastError();
+    return counted(L);
 }
-cudaError_t launch_bitrev(uint32_t* d_words, size_t nwords, int sm_count, cudaStream_t st) {
+cudaError_t launch_bitrev(LaunchCfg& L, uint32_t* d_words, size_t nwords, cudaStream_t st) {
     if (nwords == 0) return cudaSuccess;
-    k_bitrev<<<grid_for(nwords, 256, sm_count), 256, 0, st>>>(d_words, nwords);
-    return cudaGetLastError();
+    k_bitrev<<<grid_for(nwords, 256, L.sm_count), 256, 0, st>>>(d_words, nwords);
+    return counted(L);
 }
-cudaError_t launch_unpack_bits(const uint32_t* d_words, uint8_t* d_out, size_t nbits, int sm_count, cudaStream_t st) {
+cudaError_t launch_unpack_bits(LaunchCfg& L, const uint32_t* d_words, uint8_t* d_out, size_t nbits, cudaStream_t st) {
     if (nbits == 0) return cudaSuccess;
-    k_unpack_bits<<<grid_for(nbits, 256, sm_count), 256, 0, st>>>(d_words, d_out, nbits);
-    return cudaGetLastError();
+    k_unpack_bits<<<grid_for(nbits, 256, L.sm_count), 256, 0, st>>>(d_words, d_out, nbits);
+    return counted(L);
 }
-cudaError_t launch_pack_bytes(const uint8_t* d_bytes, uint32_t* d_words, size_t nbits, int sm_count, cudaStream_t st) {
+cudaError_t launch_pack_bytes(LaunchCfg& L, const uint8_t* d_bytes, uint32_t* d_words, size_t nbits, cudaStream_t st) {
     if (nbits == 0) return cudaSuccess;
-    k_pack_bytes<<<grid_for((nbits + 31) / 32, 256, sm_count), 256, 0, st>>>(d_bytes, d_words, nbits);
-    return cudaGetLastError();
+    k_pack_bytes<<<grid_for((nbits + 31) / 32, 256, L.sm_count), 256, 0, st>>>(d_bytes, d_words, nbits);
+    return counted(L);
 }
 
-cudaError_t launch_unpack_bits_msb(const uint32_t* d_words, uint8_t* d_out, size_t nbits, int sm_count, cudaStream_t st) {
+cudaError_t launch_unpack_bits_msb(LaunchCfg& L, const uint32_t* d_words, uint8_t* d_out, size_t nbits, cudaStream_t st) {
     if (nbits == 0) return cudaSuccess;
-    k_unpack_bits_msb<<<grid_for(nbits, 256, sm_count), 256, 0, st>>>(d_words, d_out, nbits);
-    return cudaGetLastError();
+    k_unpack_bits_msb<<<grid_for(nbits, 256, L.sm_count), 256, 0, st>>>(d_words, d_out, nbits);
+    return counted(L);
 }
-cudaError_t launch_popcount(const uint32_t* d_words, size_t nwords, uint32_t* d_out, int sm_count, cudaStream_t st) {
+cudaError_t launch_popcount(LaunchCfg& L, const uint32_t* d_words, size_t nwords, uint32_t* d_out, cudaStream_t st) {
     if (nwords == 0) return cudaSuccess;
-    k_popcount<<<grid_for(nwords, 256, sm_count), 256, 0, st>>>(d_words, nwords, d_out);
-    return cudaGetLastError();
+    k_popcount<<<grid_for(nwords, 256, L.sm_count), 256, 0, st>>>(d_words, nwords, d_out);
+    return counted(L);
 }
-cudaError_t launch_count_diff(const uint32_t* a, const uint32_t* b, size_t stride_words, size_t nwords, int F,
-                              uint32_t* d_out, int sm_count, cudaStream_t st) {
+cudaError_t launch_count_diff(LaunchCfg& L, const uint32_t* a, const uint32_t* b, size_t stride_words, size_t nwords, int F,
+                              uint32_t* d_out, cudaStream_t st) {
     if (nwords == 0 || F <= 0) return cudaSuccess;
-    unsigned gx = grid_for(nwords, 256, sm_count);
+    unsigned gx = grid_for(nwords, 256, L.sm_count);
     if (gx > 64u) gx = 64u;
     dim3 g(gx, (unsigned)F);
     k_count_diff<<<g, 256, 0, st>>>(a, b, stride_words, nwords, d_out);
-    return cudaGetLastError();
+    return counted(L);
 }
-cudaError_t launch_items_u32(const FrameJob* d_job, const uint32_t* d_items, uint32_t count, uint8_t* d_result, int insert, int sm_count,
-                             cudaStream_t st) {
+cudaError_t launch_items_u32(LaunchCfg& L, const FrameJob* d_job, const uint32_t* d_items, uint32_t count, uint8_t* d_result,
+                             int insert, cudaStream_t st) {
     if (count == 0) return cudaSuccess;
-    k_items_u32<<<grid_for(count, 256, sm_count), 256, 0, st>>>(d_job, d_items, count, d_result, insert);
-    return cudaGetLastError();
+    k_items_u32<<<grid_for(count, 256, L.sm_count), 256, 0, st>>>(d_job, d_items, count, d_result, insert);
+    return counted(L);
 }
-cudaError_t launch_items_str(const FrameJob* d_job, const uint8_t* d_blob, const uint64_t* d_offs, uint32_t count,
-                             uint8_t* d_result, int insert, int standard_k, int sm_count, cudaStream_t st) {
+cudaError_t launch_items_str(LaunchCfg& L, const FrameJob* d_job, const uint8_t* d_blob, const uint64_t* d_offs, uint32_t count,
+                             uint8_t* d_result, int insert, int standard_k, cudaStream_t st) {
     if (count == 0) return cudaSuccess;
-    k_items_str<<<grid_for(count, 128, sm_count), 128, 0, st>>>(d_job, d_blob, d_offs, count, d_result, insert, standard_k);
-    return cudaGetLastError();
+    k_items_str<<<grid_for(count, 128, L.sm_count), 128, 0, st>>>(d_job, d_blob, d_offs, count, d_result, insert, standard_k);
+    return counted(L);
 }
-cudaError_t launch_hash_debug(const uint32_t* d_items, uint32_t count, uint64_t seed, uint64_t* d_out, int mode, int sm_count,
+cudaError_t launch_hash_debug(LaunchCfg& L, const uint32_t* d_items, uint32_t count, uint64_t seed, uint64_t* d_out, int mode,
                               cudaStream_t st) {
     if (count == 0) return cudaSuccess;
-    k_hash_debug<<<grid_for(count, 256, sm_count), 256, 0, st>>>(d_items, count, seed, d_out, mode);
-    return cudaGetLastError();
+    k_hash_debug<<<grid_for(count, 256, L.sm_count), 256, 0, st>>>(d_items, count, seed, d_out, mode);
+    return counted(L);
 }
 
-cudaError_t launch_push_slots(const uint32_t* d_bits, size_t stride_w, uint32_t slot_w, uint32_t pairs, uint32_t* const* recv,
-                              uint32_t* const* flags, int nranks, int rank, size_t dst_off_w, uint32_t seq, int sm_count, cudaStream_t st) {
+cudaError_t launch_push_slots(LaunchCfg& L, const uint32_t* d_bits, size_t stride_w, uint32_t slot_w, uint32_t pairs,
+                              uint32_t* const* recv, uint32_t* const* flags, int nranks, int rank, size_t dst_off_w, uint32_t seq,
+                              cudaStream_t st) {
     if (nranks < 1 || nranks > PEER_MAX) return cudaErrorInvalidValue;
     PeerTable pt;
     for (int r = 0; r < PEER_MAX; r++) { pt.recv[r] = r < nranks ? recv[r] : nullptr; pt.flags[r] = r < nranks ? flags[r] : nullptr; }
     if ((slot_w & 3u) || (stride_w & 3u) || (dst_off_w & 3u)) return cudaErrorInvalidValue;
     const size_t total = (size_t)pairs * (slot_w >> 2);
     size_t grid = (total + 255) / 256;
-    if (grid > (size_t)sm_count * 8) grid = (size_t)sm_count * 8;
+    if (grid > (size_t)L.sm_count * 8) grid = (size_t)L.sm_count * 8;
     if (grid < 1) grid = 1;
     k_push_slots<<<(unsigned)grid, 256, 0, st>>>(d_bits, stride_w, slot_w, pairs, pt, nranks, dst_off_w);
     k_peer_signal<<<1, 32, 0, st>>>(pt, nranks, rank, seq);
-    return cudaGetLastError();
+    return counted(L, 2);
 }
-cudaError_t launch_peer_wait(const uint32_t* d_flags, int nranks, uint32_t seq, long long timeout_cycles, uint32_t* d_err, cudaStream_t st) {
+cudaError_t launch_peer_wait(LaunchCfg& L, const uint32_t* d_flags, int nranks, uint32_t seq, long long timeout_cycles, uint32_t* d_err,
+                             cudaStream_t st) {
     k_peer_wait<<<1, 32, 0, st>>>(d_flags, nranks, seq, timeout_cycles, d_err);
-    return cudaGetLastError();
+    return counted(L);
 }
 
 // N4: one CTA per segment; d_res: kDeflateSeg uint32 per segment of the launch
-cudaError_t launch_deflate_segments(const DeflateSeg* d_segs, int count, uint32_t* d_res, uint32_t* d_sizes, uint32_t* d_adler,
-                                    uint32_t* d_err, cudaStream_t st) {
+cudaError_t launch_deflate_segments(LaunchCfg& L, const DeflateSeg* d_segs, int count, uint32_t* d_res, uint32_t* d_sizes,
+                                    uint32_t* d_adler, uint32_t* d_err, cudaStream_t st) {
     if (count <= 0) return cudaSuccess;
     cudaError_t e = cudaFuncSetAttribute(k_deflate_segments, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDzBytes);
     if (e != cudaSuccess) return e;
     k_deflate_segments<<<count, kDeflateThreads, kDzBytes, st>>>(d_segs, d_res, d_sizes, d_adler, d_err);
-    return cudaGetLastError();
+    return counted(L);
 }
-cudaError_t launch_deflate_concat(const DeflateCopy* d_jobs, int count, uint8_t* d_dst, uint64_t cap, uint32_t* d_err, cudaStream_t st) {
+cudaError_t launch_deflate_concat(LaunchCfg& L, const DeflateCopy* d_jobs, int count, uint8_t* d_dst, uint64_t cap, uint32_t* d_err,
+                                  cudaStream_t st) {
     if (count <= 0) return cudaSuccess;
     k_deflate_concat<<<count, 256, 0, st>>>(d_jobs, d_dst, cap, d_err);
-    return cudaGetLastError();
+    return counted(L);
 }
 int deflate_code_lengths_host(const uint32_t* freqs, uint32_t nsym, uint32_t max_bits, uint8_t* lengths) {
     HuffScratch S;

@@ -88,58 +88,78 @@ struct DeflateCopy {
 };
 
 
+// What the launchers read from the context (rbf_set_option), and its kernel counter: every launcher adds the kernels it enqueued.
+struct LaunchCfg {
+    int sm_count = 0;
+    int k1_variant = 0;
+    int k1_ctas_per_sm = 32;       // grid cap of K1 (pipelined encodes use pipe_k1_ctas_per_sm so that K2 finds room beside it)
+    int pipe_k1_ctas_per_sm = 4;
+    int insert_variant = 1;        // 1: dense warp-compacted K2 building the arrays in shared memory (default); 0: per-lane K2, RED.OR into L2
+    int query_variant = 5;         // 0: per-lane; 1: staged A->B->C rings, L2 tail; 2, 3, 4: as 5; 5: decade tiles with carried stage-B
+                                   // batches (half tiles for 2^23 < m <= 2^24, ring kernel beyond); 6: half-decade tiles for every m <= 2^24
+    int query_smem_cap = 0;
+    int query_warps = 0;           // warps per CTA of the tile query kernel (0 = its compiled maximum, 28)
+    int k2_clusters[9] = {0};      // resident K2 clusters of 1..8 CTAs, measured by the first K2 launch of each shape.  Not at
+                                   // creation: querying it there slowed 8K K3 (which never uses this kernel) by 12 %, cause unknown
+    int64_t launches = 0;          // kernels enqueued (rbf_get_counter "kernel_launches")
+};
+
 // launchers (all asynchronous on `st`); return cudaError_t of the launch
-// chain: the F pairs satisfy pairs[t].curr == pairs[t+1].prev and their frames are 16 B aligned (K1 then reads each frame once)
-cudaError_t launch_threshold(const PairJob* d_pairs, int F, uint32_t npix, int channels, int sample_bytes,
-                             int thr_int, int any_mode, int gray_mode, uint32_t* d_ones, uint32_t* d_resid, int variant,
-                             bool chain, int sm_count, int ctas_per_sm, cudaStream_t st);
-// K2: variant 1 builds the arrays in (cluster) shared memory.  k2_clusters[1..8]: resident clusters of that many CTAs, 0 until
+// chain: the F pairs satisfy pairs[t].curr == pairs[t+1].prev and their frames are 16 B aligned (K1 then reads each frame once);
+// pipelined: K2 runs beside this K1, whose grid is then capped by L.pipe_k1_ctas_per_sm instead of L.k1_ctas_per_sm
+cudaError_t launch_threshold(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t npix, int channels, int sample_bytes,
+                             int thr_int, int any_mode, int gray_mode, uint32_t* d_ones, uint32_t* d_resid, bool chain, bool pipelined,
+                             cudaStream_t st);
+// K2: variant 1 builds the arrays in (cluster) shared memory.  L.k2_clusters[1..8]: resident clusters of that many CTAs, 0 until
 // the first launch of the shape measures it with cudaOccupancyMaxActiveClusters (a shape that cannot be scheduled is an error)
-cudaError_t launch_insert(const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t max_l_bits, int variant, int sm_count,
-                          int* k2_clusters, cudaStream_t st);
-cudaError_t launch_query(const FrameJob* d_jobs, const uint32_t* d_cent_prefix, int F, uint32_t total_centuries,
-                         uint32_t max_l_bits, int variant, int sm_count, int smem_bytes_cap, int tile_warps, cudaStream_t st);
-cudaError_t launch_witness(const FrameJob* d_jobs, int F, uint32_t max_centuries, int sm_count, uint32_t* d_scratch, uint32_t* d_wlen,
+cudaError_t launch_insert(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t max_l_bits, cudaStream_t st);
+cudaError_t launch_query(LaunchCfg& L, const FrameJob* d_jobs, const uint32_t* d_cent_prefix, int F, uint32_t total_centuries,
+                         uint32_t max_l_bits, cudaStream_t st);
+cudaError_t launch_witness(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t* d_scratch, uint32_t* d_wlen,
                            cudaStream_t st);
-cudaError_t launch_expand(const FrameJob* d_jobs, int F, uint32_t max_centuries, int sm_count, uint32_t* d_scratch, uint32_t* d_consumed,
+cudaError_t launch_expand(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t* d_scratch, uint32_t* d_consumed,
                           cudaStream_t st);
 uint32_t gather_chunks(uint32_t npix);
 // resid_sample_bytes: 0 gathers the current frame's samples; 1 or 2 gathers curr - prev per sample of that width (gather only,
 // pix_bytes / resid_sample_bytes channels of 1 or 3)
-cudaError_t launch_gather_scatter(const GatherJob* d_jobs, int F, int scatter, uint32_t npix, uint32_t pix_bytes, uint32_t* d_counts,
-                                  uint32_t* d_totals, cudaStream_t st, uint32_t resid_sample_bytes = 0);
+cudaError_t launch_gather_scatter(LaunchCfg& L, const GatherJob* d_jobs, int F, int scatter, uint32_t npix, uint32_t pix_bytes,
+                                  uint32_t* d_counts, uint32_t* d_totals, cudaStream_t st, uint32_t resid_sample_bytes = 0);
 // decode side of a group (rbf_k4c_apply.cuh): masks of the raw-passthrough jobs (l == 0) from their bitmap slots; set bits per mask
-cudaError_t launch_raw_masks(const FrameJob* d_jobs, int F, uint32_t npix, cudaStream_t st);
-cudaError_t launch_mask_popcount(const uint32_t* d_masks, size_t stride_w, uint32_t npix, int F, uint32_t* d_out, int sm_count,
+cudaError_t launch_raw_masks(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t npix, cudaStream_t st);
+cudaError_t launch_mask_popcount(LaunchCfg& L, const uint32_t* d_masks, size_t stride_w, uint32_t npix, int F, uint32_t* d_out,
                                  cudaStream_t st);
 // K4c: tile counts, tile scan (+ the ivc:882 check) and the chained sweep; *A.first_bad must hold UINT32_MAX before the launch.
 // A.residual == NULL runs the plain sweep, which has no residual branch at all
-cudaError_t launch_apply_chain(const ApplyChain& A, int sm_count, cudaStream_t st);
-cudaError_t launch_median5(const void* d_in, uint32_t pix_stride, uint32_t H, uint32_t W, int sample_bytes, void* d_out, cudaStream_t st);
-cudaError_t launch_bitrev(uint32_t* d_words, size_t nwords, int sm_count, cudaStream_t st);
-cudaError_t launch_unpack_bits(const uint32_t* d_words, uint8_t* d_out, size_t nbits, int sm_count, cudaStream_t st);
-cudaError_t launch_unpack_bits_msb(const uint32_t* d_words, uint8_t* d_out, size_t nbits, int sm_count, cudaStream_t st);
-cudaError_t launch_popcount(const uint32_t* d_words, size_t nwords, uint32_t* d_out, int sm_count, cudaStream_t st);
-cudaError_t launch_count_diff(const uint32_t* a, const uint32_t* b, size_t stride_words, size_t nwords, int F,
-                              uint32_t* d_out, int sm_count, cudaStream_t st);
-cudaError_t launch_pack_bytes(const uint8_t* d_bytes, uint32_t* d_words, size_t nbits, int sm_count, cudaStream_t st);
+cudaError_t launch_apply_chain(LaunchCfg& L, const ApplyChain& A, cudaStream_t st);
+cudaError_t launch_median5(LaunchCfg& L, const void* d_in, uint32_t pix_stride, uint32_t H, uint32_t W, int sample_bytes, void* d_out,
+                           cudaStream_t st);
+cudaError_t launch_bitrev(LaunchCfg& L, uint32_t* d_words, size_t nwords, cudaStream_t st);
+cudaError_t launch_unpack_bits(LaunchCfg& L, const uint32_t* d_words, uint8_t* d_out, size_t nbits, cudaStream_t st);
+cudaError_t launch_unpack_bits_msb(LaunchCfg& L, const uint32_t* d_words, uint8_t* d_out, size_t nbits, cudaStream_t st);
+cudaError_t launch_popcount(LaunchCfg& L, const uint32_t* d_words, size_t nwords, uint32_t* d_out, cudaStream_t st);
+cudaError_t launch_count_diff(LaunchCfg& L, const uint32_t* a, const uint32_t* b, size_t stride_words, size_t nwords, int F,
+                              uint32_t* d_out, cudaStream_t st);
+cudaError_t launch_pack_bytes(LaunchCfg& L, const uint8_t* d_bytes, uint32_t* d_words, size_t nbits, cudaStream_t st);
 
 // explicit-item kernels (drop-in RationalBloomFilter.add_index/check_index, rbf add/contains)
-cudaError_t launch_items_u32(const FrameJob* d_job, const uint32_t* d_items, uint32_t count, uint8_t* d_result,
-                             int insert, int sm_count, cudaStream_t st);
-cudaError_t launch_items_str(const FrameJob* d_job, const uint8_t* d_blob, const uint64_t* d_offs, uint32_t count,
-                             uint8_t* d_result, int insert, int standard_k, int sm_count, cudaStream_t st);
-cudaError_t launch_hash_debug(const uint32_t* d_items, uint32_t count, uint64_t seed, uint64_t* d_out, int mode, int sm_count,
+cudaError_t launch_items_u32(LaunchCfg& L, const FrameJob* d_job, const uint32_t* d_items, uint32_t count, uint8_t* d_result,
+                             int insert, cudaStream_t st);
+cudaError_t launch_items_str(LaunchCfg& L, const FrameJob* d_job, const uint8_t* d_blob, const uint64_t* d_offs, uint32_t count,
+                             uint8_t* d_result, int insert, int standard_k, cudaStream_t st);
+cudaError_t launch_hash_debug(LaunchCfg& L, const uint32_t* d_items, uint32_t count, uint64_t seed, uint64_t* d_out, int mode,
                               cudaStream_t st);
 
 // exchange over peer memory: store `pairs` slots of slot_w words into recv[r] + dst_off_w of every rank, then signal `seq`
-cudaError_t launch_push_slots(const uint32_t* d_bits, size_t stride_w, uint32_t slot_w, uint32_t pairs, uint32_t* const* recv,
-                              uint32_t* const* flags, int nranks, int rank, size_t dst_off_w, uint32_t seq, int sm_count, cudaStream_t st);
-cudaError_t launch_peer_wait(const uint32_t* d_flags, int nranks, uint32_t seq, long long timeout_cycles, uint32_t* d_err, cudaStream_t st);
+cudaError_t launch_push_slots(LaunchCfg& L, const uint32_t* d_bits, size_t stride_w, uint32_t slot_w, uint32_t pairs,
+                              uint32_t* const* recv, uint32_t* const* flags, int nranks, int rank, size_t dst_off_w, uint32_t seq,
+                              cudaStream_t st);
+cudaError_t launch_peer_wait(LaunchCfg& L, const uint32_t* d_flags, int nranks, uint32_t seq, long long timeout_cycles, uint32_t* d_err,
+                             cudaStream_t st);
 
-cudaError_t launch_deflate_segments(const DeflateSeg* d_segs, int count, uint32_t* d_res, uint32_t* d_sizes, uint32_t* d_adler,
-                                    uint32_t* d_err, cudaStream_t st);
-cudaError_t launch_deflate_concat(const DeflateCopy* d_jobs, int count, uint8_t* d_dst, uint64_t cap, uint32_t* d_err, cudaStream_t st);
+cudaError_t launch_deflate_segments(LaunchCfg& L, const DeflateSeg* d_segs, int count, uint32_t* d_res, uint32_t* d_sizes,
+                                    uint32_t* d_adler, uint32_t* d_err, cudaStream_t st);
+cudaError_t launch_deflate_concat(LaunchCfg& L, const DeflateCopy* d_jobs, int count, uint8_t* d_dst, uint64_t cap, uint32_t* d_err,
+                                  cudaStream_t st);
 int deflate_code_lengths_host(const uint32_t* freqs, uint32_t nsym, uint32_t max_bits, uint8_t* lengths);
 
 int query_max_smem_bytes();

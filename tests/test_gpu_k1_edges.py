@@ -285,12 +285,12 @@ def test_probe_chain_pairs(fmt):
 # ------------------------------------------------------------------ thresholds and the sizes where the kernels change course
 THRESHOLDS = [-math.inf, -1e12, -40000.5, -32769.0, -32768.5, -32768.0, -2.0, -1.5, -1.0, -0.5, 0.0, 0.5, 1.0, 126.5, 253.5,
               254.0, 254.5, 255.0, 256.0, 32767.0, 32768.0, 65535.0, 1e9, 1e12, math.inf, math.nan]
-# one threshold per branch of threshold_to_int / stream_thr_int / k1_thr, for the size sweeps and the big frames
+# one threshold per branch of threshold_to_int / k1_thr, for the size sweeps and the big frames
 EDGE_THRESHOLDS = [-math.inf, -32768.5, -32768.0, -1.0, 0.0, 126.5, 254.0, 255.0, 32767.0, 1e12, math.nan]
 
 
 def test_threshold_lists_reach_every_branch():
-    """threshold_to_int: NaN, < -1, > 1e9, floor; stream_thr_int (16-bit, < -1): < -40000, floor; k1_thr: < 0, 0..254, > 254."""
+    """threshold_to_int: NaN, < -1 (16-bit: < -40000, floor), > 1e9, floor; k1_thr: < 0, 0..254, > 254."""
     for ths in (THRESHOLDS, EDGE_THRESHOLDS):
         assert any(math.isnan(t) for t in ths)
         assert any(t < -40000 for t in ths) and any(-40000 <= t < -1 for t in ths)
