@@ -818,6 +818,8 @@ static void stream_range_params(rbf_stream* s, uint32_t first, uint32_t count, c
 // array at or beyond bit l, or a witness at or beyond bit wlen, and both regions are fully zeroed at creation, so clearing
 // [0, high-water mark) of every slot is enough.  Keep the work list behind the jobs: uploaded ahead of them, it held K2 of
 // rbf_stream_encode_host's first chunk until every frame copy of the call had landed (+20 ms per 4K call on an H100 at 700 W).
+// Every range and chunk of an encode is staged, whether or not it has a coded pair, so that after any encode a raw pair's rows read
+// as zero and K3b never sees a job of an earlier call.  Copies and memsets only: kernel_launches does not count this step.
 static int enc_stage_jobs(rbf_stream* s, uint32_t f, uint32_t cnt, uint32_t max_l, const uint32_t* hp) {
     rbf_ctx* c = s->c;
     CK(c, cudaMemcpyAsync(s->d_jobs + f, s->h_jobs + f, sizeof(FrameJob) * cnt, cudaMemcpyHostToDevice, c->st));
@@ -887,8 +889,8 @@ static int stream_encode_range(rbf_stream* s, uint32_t first, uint32_t count, ui
     RangeTotals rt;
     uint32_t* hp = s->h_prefix + pfx;
     stream_range_params(s, first, count, sd, nullptr, nullptr, hp, 0, &rt);
+    if (int r = enc_stage_jobs(s, first, count, rt.max_l, hp)) return r;   // also when all raw: the caller copies these rows out
     if (rt.coded_pairs == 0) return RBF_OK;
-    if (int r = enc_stage_jobs(s, first, count, rt.max_l, hp)) return r;
     CK(c, launch_insert(c->L, s->d_jobs + first, (int)count, (uint32_t)((s->npix + 99) / 100), rt.max_l, c->st));
     CK(c, launch_query(c->L, s->d_jobs + first, s->d_prefix + pfx, (int)count, rt.total_cent, rt.max_l, c->st));
     return enc_witness(s, first, count, false);
@@ -942,14 +944,16 @@ static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t
     for (uint32_t r = 0; r < R; r++) {
         const uint32_t f = lo[r], cnt = lo[r + 1] - lo[r];
         CK(c, cudaEventSynchronize(c->ev_k1[r]));         // this range's counts are on the host
-        RangeTotals rt;
-        stream_range_params(s, f, cnt, sd, kov, lov, s->h_prefix + f, base_cent, &rt);
+        RangeTotals rt;                                    // the overrides are per pair: range r reads entries [f, f+cnt)
+        stream_range_params(s, f, cnt, sd, kov ? kov + f : nullptr, lov ? lov + f : nullptr, s->h_prefix + f, base_cent, &rt);
         base_cent += rt.total_cent;
         all.coded_pairs += rt.coded_pairs;
         if (rt.max_l > all.max_l) all.max_l = rt.max_l;
-        if (s->k1_only || rt.coded_pairs == 0) continue;
+        if (s->k1_only) continue;
         CK(c, cudaStreamWaitEvent(c->st, c->ev_k1[r], 0)); // K2 reads the masks K1 wrote on the other stream
+        // a range without a coded pair is staged too: K3b runs over every pair's job, and its raw rows must read as zero
         if (int e = enc_stage_jobs(s, f, cnt, rt.max_l, nullptr)) return e;   // the work list goes up once, for all ranges
+        if (rt.coded_pairs == 0) continue;
         if (first_k2) { CK(c, cudaEventRecord(s->ev[2], c->st)); first_k2 = false; }
         if (!kq) CK(c, launch_insert(c->L, s->d_jobs + f, (int)cnt, ncent, rt.max_l, c->st));
     }
