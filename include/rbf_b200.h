@@ -150,7 +150,11 @@ void rbf_stream_destroy(rbf_stream* s);
  *               OpenCV's fixed point (3735 B + 19235 G + 9798 R + 16384) >> 15 for 8- and 16-bit samples
  *   "value_mode" what rbf_stream_gather_changed and rbf_stream_zlib_changed return per changed pixel: 0 (default) the current
  *               frame's samples; 1 residuals (curr - prev) mod 2^(8 sample_bytes) per sample, little-endian, in the same order
- *               and count.  1 needs 1 or 3 channels of 1- or 2-byte samples; other values or shapes are RBF_ERR_INVALID */
+ *               and count.  1 needs 1 or 3 channels of 1- or 2-byte samples; other values or shapes are RBF_ERR_INVALID
+ *   "motion_values" 1: the same gathers return residuals against the motion-compensated previous frame of each pair,
+ *               (curr - pred) mod 2^(8 sample_bytes) per sample, pred as in rbf_stream_motion_search with the fields of the last
+ *               search.  RBF_ERR_INVALID when no search has run since the last encode or when value_mode is 1 (value_mode 1 is
+ *               likewise refused while motion_values is 1); a gather of more pairs than were searched fails too */
 int rbf_stream_set_option(rbf_stream* s, const char* key, int64_t value);
 int rbf_stream_upload(rbf_stream* s, uint32_t first_frame, uint32_t count, const void* host_frames);
 int rbf_stream_frame_ptr(rbf_stream* s, uint32_t frame, void** dptr);
@@ -213,6 +217,14 @@ int rbf_stream_download(rbf_stream* s, uint32_t frame, void* host_out);
  *     of replacing them; 0 means plain values.  residual may be NULL (every pair plain: rbf_stream_apply_chain itself); a flag
  *     other than 0 or 1 is RBF_ERR_INVALID.  The flags travel in the same H2D copy as the offsets; ivc:882, the first-bad-pair
  *     rule and slot wrap-around are the same for both kinds.
+ * rbf_stream_apply_chain_motion  rbf_stream_apply_chain_modes with a third mode: modes[i] == 2 means pair i's values are residuals
+ *     against the motion-compensated frame base_frame+i (what a gather with motion_values 1 returns), added per sample to
+ *     pred(y, x) = frame(clamp(y + dy), clamp(x + dx)) at the selected pixels; the other pixels are copied.  fields holds
+ *     count x mv_blocks x 2 int8 (dx, dy per 16 x 16 block, raster order; what rbf_stream_motion_search returns), one field per
+ *     pair, read for mode 2 pairs only; it may be NULL when no pair has mode 2.  A mode above 2 or a vector component outside
+ *     [-16, 16] is RBF_ERR_INVALID before anything is launched.  The modes and fields travel in the same H2D copy as the offsets.
+ *     Runs of mode 0 / 1 pairs are applied by one K4c sweep each, every mode 2 pair by its own kernel, behind one tile count and
+ *     scan for the whole chain on one CUDA stream; ivc:882, the first-bad-pair rule and slot wrap-around hold as above.
  * rbf_stream_download_batch  frames first .. first+count-1 (slots modulo max_frames) into one contiguous host array, one
  *     synchronisation. */
 int rbf_stream_decode_masks(rbf_stream* s, uint32_t count, const uint8_t* bitmaps_packbits, uint64_t bitmap_slot_bytes,
@@ -222,6 +234,15 @@ int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32_t count, c
                            uint64_t* applied_out);
 int rbf_stream_apply_chain_modes(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
                                  const uint64_t* value_offsets, const uint8_t* residual /* [count] or NULL */, uint64_t* applied_out);
+int rbf_stream_apply_chain_motion(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
+                                  const uint64_t* value_offsets, const uint8_t* modes /* [count] */,
+                                  const int8_t* fields /* [count][mv_blocks][2] or NULL */, uint64_t* applied_out);
+/* Block motion search of pairs [0, pairs) of the last encode, prev -> curr: 16 x 16 blocks in raster order (mv_blocks =
+ * ceil(H/16) x ceil(W/16), edge blocks clipped to the frame); per block the (dx, dy) in [-16, 16]^2 that minimises the SAD over the
+ * block's pixels and samples of |curr - pred|, pred(y, x) = prev(clamp(y + dy, 0, H-1), clamp(x + dx, 0, W-1)); ties go to the
+ * smaller |dx| + |dy|, then the smaller dy, then the smaller dx.  fields_out[pairs][mv_blocks][2] = int8 dx, dy; the fields also
+ * stay in the stream for the motion_values gathers until the next encode or rbf_stream_decode_masks.  One synchronisation. */
+int rbf_stream_motion_search(rbf_stream* s, uint32_t pairs, int8_t* fields_out);
 int rbf_stream_download_batch(rbf_stream* s, uint32_t first, uint32_t count, void* host_out);
 /* N3  the 5x5 median of cv2.medianBlur in VideoFrameCompressor._estimate_noise_level (ivc:738): replicated border, 13th
  *     smallest of 25, exact for uint8 / uint16.  The float32 std of (frame - median) stays in numpy (ivc:741-744). */

@@ -49,7 +49,8 @@ EXPORTS = [
     "rbf_stream_create", "rbf_stream_destroy", "rbf_stream_set_option", "rbf_stream_upload", "rbf_stream_frame_ptr", "rbf_stream_encode",
     "rbf_stream_encode_host", "rbf_stream_fetch", "rbf_stream_fetch_batch", "rbf_stream_decode_verify", "rbf_stream_bitmap_region", "rbf_stream_stage_ms",
     "rbf_stream_gather_changed", "rbf_stream_apply_diff", "rbf_stream_download", "rbf_median_blur5", "rbf_stream_median5",
-    "rbf_stream_decode_masks", "rbf_stream_apply_chain", "rbf_stream_apply_chain_modes", "rbf_stream_download_batch",
+    "rbf_stream_decode_masks", "rbf_stream_apply_chain", "rbf_stream_apply_chain_modes", "rbf_stream_apply_chain_motion",
+    "rbf_stream_motion_search", "rbf_stream_download_batch",
     "rbf_zlib_bound", "rbf_deflate_code_lengths", "rbf_zlib_compress_batch", "rbf_stream_zlib_changed",
     "rbf_nccl_unique_id", "rbf_nccl_init", "rbf_nccl_allgather", "rbf_stream_allgather_bitmaps", "rbf_nccl_destroy",
     "rbf_peer_export", "rbf_peer_open", "rbf_peer_close", "rbf_peer_gather_init", "rbf_peer_gather_half", "rbf_peer_gather_shutdown",
@@ -122,6 +123,8 @@ def _sig(L):
     L.rbf_stream_decode_masks.argtypes = [vp, u32, vp, u64, vp, u64, vp, vp, vp, vp, P(Seeds), vp, vp]
     L.rbf_stream_apply_chain.argtypes = [vp, u32, u32, vp, vp, vp]
     L.rbf_stream_apply_chain_modes.argtypes = [vp, u32, u32, vp, vp, vp, vp]
+    L.rbf_stream_apply_chain_motion.argtypes = [vp, u32, u32, vp, vp, vp, vp, vp]
+    L.rbf_stream_motion_search.argtypes = [vp, u32, vp]
     L.rbf_stream_download_batch.argtypes = [vp, u32, u32, vp]
     L.rbf_median_blur5.argtypes = [vp, vp, u32, u32, u32, vp]
     L.rbf_stream_median5.argtypes = [vp, u32, vp]

@@ -610,6 +610,9 @@ struct rbf_stream {
     int mask_mode = 0;      // 0: |dY| > thr (ivc:808); 1: additionally any byte of the pixel differs
     int gray_mode = 0;      // 1: the mask is taken on cv2.COLOR_BGR2GRAY of the pixel (ivc:792-795) instead of on sample 0
     int value_mode = 0;     // changed-value gathers: 0 the current samples; 1 residuals (curr - prev) mod 2^(8 S) per sample
+    int motion_values = 0;  // 1: the gathers return residuals against the motion-compensated previous frame of the last search
+    int8_t* d_fields = nullptr;             // [max_pairs][mv_blocks(H, W)][2] block vectors of rbf_stream_motion_search
+    uint32_t motion_pairs = 0;              // pairs searched since the last encode (0: none, or a decode_masks overwrote the slots)
     bool last_k1_only = false;
     rbf_seeds last_sd = {};                 // seeds of the last encode (decode_verify rebuilds its jobs from them and last_infos)
     size_t bits_hwm = 0, wit_hwm = 0;   // bytes per slot that may hold set bits (see enc_stage_jobs)
@@ -623,6 +626,7 @@ extern "C" void rbf_stream_destroy(rbf_stream* s) {
     cudaSetDevice(s->c->device);
     cudaFree(s->d_frames); cudaFree(s->d_mask); cudaFree(s->d_bits); cudaFree(s->d_wit); cudaFree(s->d_pass); cudaFree(s->d_dec);
     cudaFree(s->d_jobs); cudaFree(s->d_pairs); cudaFree(s->d_prefix); cudaFree(s->d_ones); cudaFree(s->d_resid); cudaFree(s->d_wlen); cudaFree(s->d_chunkcnt);
+    cudaFree(s->d_fields);
     for (auto& e : s->ev) if (e) cudaEventDestroy(e);
     for (auto& e : s->ev_copy) if (e) cudaEventDestroy(e);
     cudaFreeHost(s->h_jobs); cudaFreeHost(s->h_pairs); cudaFreeHost(s->h_prefix); cudaFreeHost(s->h_ones); cudaFreeHost(s->h_resid); cudaFreeHost(s->h_wlen);
@@ -692,7 +696,15 @@ extern "C" int rbf_stream_set_option(rbf_stream* s, const char* key, int64_t v) 
         if (v != 0 && v != 1) return set_err(s->c, RBF_ERR_INVALID, "value_mode must be 0 (values) or 1 (residuals), not %lld", (long long)v);
         if (v && !((s->C == 1 || s->C == 3) && (s->S == 1 || s->S == 2)))
             return set_err(s->c, RBF_ERR_INVALID, "residual values need 1 or 3 channels of 8- or 16-bit samples (C=%u S=%u)", s->C, s->S);
+        if (v && s->motion_values) return set_err(s->c, RBF_ERR_INVALID, "value_mode 1 and motion_values 1 exclude each other");
         s->value_mode = (int)v;
+        return RBF_OK;
+    }
+    if (!strcmp(key, "motion_values")) {
+        if (v != 0 && v != 1) return set_err(s->c, RBF_ERR_INVALID, "motion_values must be 0 or 1, not %lld", (long long)v);
+        if (v && s->value_mode) return set_err(s->c, RBF_ERR_INVALID, "value_mode 1 and motion_values 1 exclude each other");
+        if (v && s->motion_pairs == 0) return set_err(s->c, RBF_ERR_INVALID, "motion_values needs a motion search since the last encode");
+        s->motion_values = (int)v;
         return RBF_OK;
     }
     return set_err(s->c, RBF_ERR_INVALID, "unknown stream option %s", key);
@@ -853,6 +865,7 @@ static int enc_witness(rbf_stream* s, uint32_t f, uint32_t cnt, bool timed) {
 static void enc_begin(rbf_stream* s, const rbf_seeds* sd) {
     s->last_infos.clear();
     s->last_pairs = 0; s->last_max_l = 0;
+    s->motion_pairs = 0;
     s->staged = false;
     s->last_sd = *sd;
 }
@@ -1161,10 +1174,13 @@ static uint64_t changed_offsets(const rbf_stream* s, uint32_t pairs, uint64_t* o
 }
 
 // The changed values of the encoded pairs [0, pairs) gathered at offs into the values scratch slot, on the context's stream
-// (value_mode 1: residuals against each pair's previous frame).
+// (value_mode 1: residuals against each pair's previous frame; motion_values 1: against its motion-compensated previous frame).
 static int gather_values(rbf_stream* s, uint32_t pairs, const uint64_t* offs, uint8_t** d_values) {
     rbf_ctx* c = s->c;
     const uint32_t pb = s->C * s->S;
+    if (s->motion_values && pairs > s->motion_pairs)
+        return set_err(c, RBF_ERR_INVALID, "motion_values: %u pairs were searched since the last encode, %u are gathered", s->motion_pairs, pairs);
+    const size_t field_bytes = (size_t)mv_blocks(s->H, s->W) * 2;
     void *d_vals = nullptr, *d_jobs = nullptr, *d_gcnt = nullptr;
     int rc;
     if ((rc = scratch_get(c, kScrValues, (size_t)offs[pairs] + 256, &d_vals)) ||
@@ -1181,10 +1197,12 @@ static int gather_values(rbf_stream* s, uint32_t pairs, const uint64_t* offs, ui
         J.out_frame = nullptr;
         J.npix = (uint32_t)s->npix;
         J.pix_bytes = pb;
+        J.width = s->W;
+        J.field = s->motion_values ? s->d_fields + i * field_bytes : nullptr;
     }
     CK(c, cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(GatherJob) * pairs, cudaMemcpyHostToDevice, c->st));   // pageable: staged before return
     CK(c, launch_gather_scatter(c->L, (const GatherJob*)d_jobs, (int)pairs, 0, (uint32_t)s->npix, pb, (uint32_t*)d_gcnt, nullptr, c->st,
-                                s->value_mode ? s->S : 0u));
+                                s->value_mode || s->motion_values ? s->S : 0u, s->motion_values != 0));
     *d_values = (uint8_t*)d_vals;
     return RBF_OK;
 }
@@ -1227,7 +1245,7 @@ extern "C" int rbf_stream_apply_diff(rbf_stream* s, uint32_t base_frame, uint32_
         CK(c, cudaMemcpyAsync(dst, s->d_frames + (size_t)base_frame * s->frame_stride, s->frame_bytes, cudaMemcpyDeviceToDevice, c->st));
     GatherJob J;
     J.mask = (const uint32_t*)d_mask; J.frame = nullptr; J.values = (uint8_t*)d_vals; J.out_frame = dst;
-    J.npix = (uint32_t)s->npix; J.pix_bytes = (uint32_t)pb;
+    J.npix = (uint32_t)s->npix; J.pix_bytes = (uint32_t)pb; J.width = s->W; J.field = nullptr;
     uint32_t* d_cnt = (uint32_t*)((uint8_t*)d_job + sizeof(GatherJob));
     // the reference applies the diff only when the value count matches the mask (ivc:882): count first
     CK(c, cudaMemsetAsync(d_cnt, 0, 4, c->st));
@@ -1318,7 +1336,7 @@ extern "C" int rbf_stream_decode_masks(rbf_stream* s, uint32_t count, const uint
     for (uint32_t i = 0; i < count; i++) { consumed_out[i] = raw[i] ? 0 : h[i]; ones_out[i] = h[count + i]; }
     // the slots no longer hold the outputs of an encode: refuse fetch / gather / decode_verify until the next one, and let the next
     // encode clear what was written here
-    s->last_pairs = 0; s->last_max_l = 0; s->staged = false;
+    s->last_pairs = 0; s->last_max_l = 0; s->staged = false; s->motion_pairs = 0;
     const size_t bh = align_up((size_t)bitmap_slot + 64, 128), wh = align_up((size_t)witness_slot + 64, 128);
     if (bh > s->bits_hwm) s->bits_hwm = bh;
     if (witness_slot && wh > s->wit_hwm) s->wit_hwm = wh;
@@ -1330,8 +1348,9 @@ extern "C" int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32
     return rbf_stream_apply_chain_modes(s, base_frame, count, values, value_offsets, nullptr, applied_out);
 }
 
-extern "C" int rbf_stream_apply_chain_modes(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
-                                            const uint64_t* value_offsets, const uint8_t* residual, uint64_t* applied_out) {
+// rbf_stream_apply_chain_modes / _motion: modes[i] <= max_mode (NULL: every pair plain); fields [count][nblocks][2] for mode 2 pairs
+static int apply_chain_impl(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values, const uint64_t* value_offsets,
+                            const uint8_t* modes, uint8_t max_mode, const int8_t* fields, uint64_t* applied_out) {
     if (!s || !value_offsets || !applied_out) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_apply_chain: NULL");
     rbf_ctx* c = s->c;
     if (count == 0 || count > s->max_pairs || count >= s->max_frames || base_frame >= s->max_frames)
@@ -1339,35 +1358,46 @@ extern "C" int rbf_stream_apply_chain_modes(rbf_stream* s, uint32_t base_frame, 
                        base_frame, s->max_frames, s->max_pairs);
     for (uint32_t i = 0; i < count; i++)
         if (value_offsets[i + 1] < value_offsets[i]) return set_err(c, RBF_ERR_INVALID, "value offsets decrease at pair %u", i);
-    bool any_residual = false;
-    for (uint32_t i = 0; residual && i < count; i++) {
-        if (residual[i] > 1) return set_err(c, RBF_ERR_INVALID, "pair %u: residual flag %u is neither 0 nor 1", i, (unsigned)residual[i]);
-        any_residual |= residual[i] != 0;
+    bool any_residual = false, any_motion = false;
+    for (uint32_t i = 0; modes && i < count; i++) {
+        if (modes[i] > max_mode)
+            return set_err(c, RBF_ERR_INVALID, max_mode == 1 ? "pair %u: residual flag %u is neither 0 nor 1" : "pair %u: value mode %u is not 0, 1 or 2",
+                           i, (unsigned)modes[i]);
+        any_residual |= modes[i] == 1;
+        any_motion |= modes[i] == 2;
     }
+    const size_t field_bytes = fields ? (size_t)count * mv_blocks(s->H, s->W) * 2 : 0;
+    if (any_motion && !fields) return set_err(c, RBF_ERR_INVALID, "rbf_stream_apply_chain_motion: motion pairs without fields");
+    for (size_t i = 0; i < field_bytes; i++)
+        if (fields[i] < -MV_RANGE || fields[i] > MV_RANGE)
+            return set_err(c, RBF_ERR_INVALID, "pair %llu: motion vector component %d is outside [-%d, %d]",
+                           (unsigned long long)(i / (field_bytes / count)), (int)fields[i], MV_RANGE, MV_RANGE);
     const uint64_t vbytes = value_offsets[count];
     if (vbytes && !values) return set_err(c, RBF_ERR_INVALID, "rbf_stream_apply_chain: values is NULL");
     CK(c, cudaSetDevice(c->device));
     const uint32_t ntiles = (uint32_t)((s->npix + AP_TILE_PX - 1) / AP_TILE_PX);
     void *d_vals, *d_small, *d_pfx;
     int rc;
-    // d_small: the value offsets, then the residual flags (one H2D copy for both), then first_bad and the totals
-    const size_t off_bytes = 8 * ((size_t)count + 1), flag_bytes = residual ? count : 0, res_at = align_up(off_bytes + flag_bytes, 16);
-    const size_t small = res_at + 4 * ((size_t)count + 1);
+    // d_small: the value offsets, then the modes, then the fields (one H2D copy for all three), then first_bad and the totals
+    const size_t off_bytes = 8 * ((size_t)count + 1), flag_bytes = modes ? count : 0;
+    const size_t res_at = align_up(off_bytes + flag_bytes + field_bytes, 16);
+    const size_t small = res_at + 4 * ((size_t)count + 1) + (field_bytes ? 4 * (size_t)count : 0);   // + the runs' first_bad words
     if ((rc = scratch_get(c, kScrValues, (size_t)vbytes + 256, &d_vals)) || (rc = scratch_get(c, kScrChainSmall, small, &d_small)) ||
         (rc = scratch_get(c, kScrChainTiles, 4 * (size_t)count * ntiles, &d_pfx)))
         return rc;
     uint64_t* d_off = (uint64_t*)d_small;
     uint32_t* d_res = (uint32_t*)((uint8_t*)d_small + res_at);   // [0] first_bad, [1 + i] totals
     if (vbytes) { CK(c, cudaMemcpyAsync(d_vals, values, (size_t)vbytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)vbytes; }
-    if (residual) {
-        std::vector<uint8_t> head(off_bytes + flag_bytes);
+    if (modes) {
+        std::vector<uint8_t> head(off_bytes + flag_bytes + field_bytes);
         memcpy(head.data(), value_offsets, off_bytes);
-        memcpy(head.data() + off_bytes, residual, flag_bytes);
+        memcpy(head.data() + off_bytes, modes, flag_bytes);
+        if (field_bytes) memcpy(head.data() + off_bytes + flag_bytes, fields, field_bytes);
         CK(c, cudaMemcpyAsync(d_off, head.data(), head.size(), cudaMemcpyHostToDevice, c->st));   // pageable: staged before return
     } else {
         CK(c, cudaMemcpyAsync(d_off, value_offsets, off_bytes, cudaMemcpyHostToDevice, c->st));
     }
-    c->h2d += (int64_t)(off_bytes + flag_bytes);
+    c->h2d += (int64_t)(off_bytes + flag_bytes + field_bytes);
     CK(c, cudaMemsetAsync(d_res, 0xff, 4, c->st));
     ApplyChain A;
     A.masks = s->d_mask; A.mask_stride_w = s->mask_stride_w;
@@ -1375,15 +1405,52 @@ extern "C" int rbf_stream_apply_chain_modes(rbf_stream* s, uint32_t base_frame, 
     A.max_frames = s->max_frames; A.base = base_frame;
     A.npix = (uint32_t)s->npix; A.ntiles = ntiles; A.count = count; A.pix_bytes = s->C * s->S;
     A.values = (const uint8_t*)d_vals; A.value_off = d_off;
-    A.residual = any_residual ? (const uint8_t*)d_small + off_bytes : nullptr;   // a group without residual pairs runs the plain sweep
     A.sample_bytes = s->S;
     A.tile_pfx = (uint32_t*)d_pfx; A.totals = d_res + 1; A.first_bad = d_res;
-    CK(c, launch_apply_chain(c->L, A, c->st));
+    if (any_motion) {                                    // split at the motion pairs
+        A.residual = (const uint8_t*)d_small + off_bytes;
+        CK(c, launch_apply_chain_motion(c->L, A, modes, (const int8_t*)d_small + off_bytes + flag_bytes, s->H, s->W,
+                                        d_res + 1 + count, c->st));
+    } else {
+        A.residual = any_residual ? (const uint8_t*)d_small + off_bytes : nullptr;   // a group without residual pairs runs the plain sweep
+        CK(c, launch_apply_chain(c->L, A, c->st));
+    }
     std::vector<uint32_t> h((size_t)count + 1);
     CK(c, cudaMemcpyAsync(h.data(), d_res, 4 * ((size_t)count + 1), cudaMemcpyDeviceToHost, c->st));
     c->d2h += 4 * ((int64_t)count + 1);
     CK(c, cudaStreamSynchronize(c->st));
     for (uint32_t i = 0; i < count; i++) applied_out[i] = i < h[0] ? h[1 + i] : 0;
+    return RBF_OK;
+}
+
+extern "C" int rbf_stream_apply_chain_modes(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
+                                            const uint64_t* value_offsets, const uint8_t* residual, uint64_t* applied_out) {
+    return apply_chain_impl(s, base_frame, count, values, value_offsets, residual, 1, nullptr, applied_out);
+}
+
+extern "C" int rbf_stream_apply_chain_motion(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
+                                             const uint64_t* value_offsets, const uint8_t* modes, const int8_t* fields,
+                                             uint64_t* applied_out) {
+    if (!modes) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_apply_chain_motion: modes is NULL");
+    return apply_chain_impl(s, base_frame, count, values, value_offsets, modes, 2, fields, applied_out);
+}
+
+// ------------------------------------------------------------------------------------------
+// Block motion search of the encoded pairs (value_coding "motion"); the fields stay in the stream for the motion_values gathers
+// ------------------------------------------------------------------------------------------
+extern "C" int rbf_stream_motion_search(rbf_stream* s, uint32_t pairs, int8_t* fields_out) {
+    if (!s || !fields_out) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_motion_search: NULL");
+    rbf_ctx* c = s->c;
+    if (pairs == 0 || pairs > s->last_pairs) return set_err(c, RBF_ERR_INVALID, "only %u pairs were encoded", s->last_pairs);
+    CK(c, cudaSetDevice(c->device));
+    const size_t field_bytes = (size_t)mv_blocks(s->H, s->W) * 2;
+    if (!s->d_fields) CK(c, cudaMalloc((void**)&s->d_fields, field_bytes * s->max_pairs));
+    // the PairJobs of the last encode are still on the device (d_pairs)
+    CK(c, launch_motion_search(c->L, s->d_pairs, (int)pairs, s->H, s->W, s->C * s->S, s->S, s->d_fields, c->st));
+    CK(c, cudaMemcpyAsync(fields_out, s->d_fields, field_bytes * pairs, cudaMemcpyDeviceToHost, c->st));
+    c->d2h += (int64_t)(field_bytes * pairs);
+    CK(c, cudaStreamSynchronize(c->st));
+    s->motion_pairs = pairs;
     return RBF_OK;
 }
 

@@ -67,11 +67,23 @@ __device__ __forceinline__ void add_pixel(uint8_t* __restrict__ dst, const uint8
     }
 }
 
-// RS = 0: plain gather / scatter of the pixels; RS = 1 or 2: the gather stores residuals against J.prev per sample of RS bytes
-template <int PB, int RS>
+// Pixel index of the motion-compensated prediction of pixel px: the pixel its block's (dx, dy) points at, clamped to the frame.
+__device__ __forceinline__ size_t motion_src(const int8_t* __restrict__ field, uint32_t W, uint32_t H, uint32_t px) {
+    const uint32_t y = px / W, x = px - y * W;
+    const uint32_t b = (y / MV_BLOCK) * mv_blocks_x(W) + x / MV_BLOCK;
+    const int dx = __ldg(field + 2 * b), dy = __ldg(field + 2 * b + 1);
+    const int yy = min(max((int)y + dy, 0), (int)H - 1), xx = min(max((int)x + dx, 0), (int)W - 1);
+    return (size_t)yy * W + (uint32_t)xx;
+}
+
+// RS = 0: plain gather / scatter of the pixels; RS = 1 or 2: the gather stores residuals against J.prev per sample of RS bytes;
+// MC: against the motion-compensated J.prev (J.field, J.width) instead of the co-located pixel
+template <int PB, int RS, bool MC = false>
 __global__ void __launch_bounds__(1024) k_gather_scatter(const GatherJob* __restrict__ jobs, int scatter, uint32_t chunks,
                                                           const uint32_t* __restrict__ counts, uint32_t* __restrict__ totals) {
+    static_assert(!MC || RS != 0, "motion gathers are residual gathers");
     const GatherJob J = jobs[blockIdx.y];
+    [[maybe_unused]] const uint32_t H = MC ? J.npix / J.width : 0u;
     __shared__ uint32_t s_warp[33];
     const uint32_t nwords = (J.npix + 31u) >> 5;
     const uint32_t w_begin = (uint32_t)(((uint64_t)nwords * blockIdx.x) / chunks), w_end = (uint32_t)(((uint64_t)nwords * (blockIdx.x + 1)) / chunks);
@@ -86,7 +98,8 @@ __global__ void __launch_bounds__(1024) k_gather_scatter(const GatherJob* __rest
             const uint32_t b = __ffs(m) - 1;
             m &= m - 1u;
             const size_t px = ((size_t)w << 5) + b;
-            if constexpr (RS != 0) resid_pixel<PB, RS>(J.values + (size_t)rank * PB, J.frame + px * PB, J.prev + px * PB);
+            if constexpr (MC) resid_pixel<PB, RS>(J.values + (size_t)rank * PB, J.frame + px * PB, J.prev + motion_src(J.field, J.width, H, (uint32_t)px) * PB);
+            else if constexpr (RS != 0) resid_pixel<PB, RS>(J.values + (size_t)rank * PB, J.frame + px * PB, J.prev + px * PB);
             else if (scatter) copy_pixel<PB>(J.out_frame + px * PB, J.values + (size_t)rank * PB);
             else copy_pixel<PB>(J.values + (size_t)rank * PB, J.frame + px * PB);
             rank++;

@@ -7,6 +7,8 @@
 //   K3b k_witness        ordered witness = mask bits at passing positions           (ivc:253)
 //   K4b k_expand         decode: out[i] = witness[rank(i)] for passing i            (ivc:299-304)
 //   K4c k_apply_sweep    a group's decoded masks applied along the frame chain      (ivc:849-909)
+//   K5  k_motion_search  16 x 16 block motion search, +-16 px (value_coding "motion")
+//       k_apply_motion   a motion-compensated residual pair of a decoded group
 //   N4  k_deflate_segments / k_deflate_concat   zlib streams of host or device buffers (rbf_deflate.cuh)
 //
 // The Bloom bit array of the frame being queried is staged into shared memory with
@@ -14,7 +16,7 @@
 // CTA is probed through L2.  Integer hashing / bit tests only: no tensor cores.
 //
 // One translation unit: this file holds the PTX helpers and the launchers; the kernels live in
-// rbf_k1_threshold.cuh, rbf_k2_insert.cuh, rbf_k3_query.cuh, rbf_k3b_witness.cuh, rbf_aux_kernels.cuh, rbf_deflate.cuh and rbf_k4c_apply.cuh.
+// rbf_k1_threshold.cuh, rbf_k2_insert.cuh, rbf_k3_query.cuh, rbf_k3b_witness.cuh, rbf_aux_kernels.cuh, rbf_deflate.cuh, rbf_k4c_apply.cuh and rbf_motion.cuh.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -110,6 +112,7 @@ __device__ __forceinline__ void or_bits128(uint32_t* __restrict__ W, uint64_t bi
 #include "rbf_aux_kernels.cuh"
 #include "rbf_deflate.cuh"
 #include "rbf_k4c_apply.cuh"
+#include "rbf_motion.cuh"
 
 // ------------------------------------------------------------------------------------------
 // launchers
@@ -374,15 +377,25 @@ uint32_t gather_chunks(uint32_t npix) {
 }
 // d_counts: F * gather_chunks(npix) uint32 of scratch; d_totals (may be NULL): set pixels per pair
 cudaError_t launch_gather_scatter(LaunchCfg& L, const GatherJob* d_jobs, int F, int scatter, uint32_t npix, uint32_t pix_bytes,
-                                  uint32_t* d_counts, uint32_t* d_totals, cudaStream_t st, uint32_t resid_sample_bytes) {
+                                  uint32_t* d_counts, uint32_t* d_totals, cudaStream_t st, uint32_t resid_sample_bytes, bool motion) {
     if (F <= 0) return cudaSuccess;
     // the kernel is picked by (pixel bytes, residual sample bytes): 2 B per pixel is one 16-bit sample, never two 8-bit ones
     const uint32_t key = pix_bytes * 4u + resid_sample_bytes;
-    if (resid_sample_bytes && (scatter || !(key == 1u * 4 + 1 || key == 3u * 4 + 1 || key == 2u * 4 + 2 || key == 6u * 4 + 2)))
+    if ((resid_sample_bytes || motion) &&
+        (scatter || !(key == 1u * 4 + 1 || key == 3u * 4 + 1 || key == 2u * 4 + 2 || key == 6u * 4 + 2)))
         return cudaErrorInvalidValue;                                 // checked before anything is launched
     const uint32_t ch = gather_chunks(npix);
     const dim3 grid(ch, (unsigned)F);
     k_mask_chunk_count<<<grid, 256, 0, st>>>(d_jobs, ch, d_counts);
+    if (motion) {
+        switch (key) {
+        case 1u * 4 + 1: k_gather_scatter<1, 1, true><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;
+        case 3u * 4 + 1: k_gather_scatter<3, 1, true><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;
+        case 2u * 4 + 2: k_gather_scatter<2, 2, true><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;
+        default: k_gather_scatter<6, 2, true><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;
+        }
+        return counted(L, 2);
+    }
     switch (key) {
     case 1u * 4: k_gather_scatter<1, 0><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
     case 2u * 4: k_gather_scatter<2, 0><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
@@ -423,16 +436,12 @@ static cudaError_t launch_apply_sweep_t(LaunchCfg& L, const ApplyChain& A, cudaS
     k_apply_sweep<PB, RS><<<(A.ntiles + rounds - 1u) / rounds, AP_THREADS, 0, st>>>(A);
     return counted(L);
 }
-cudaError_t launch_apply_chain(LaunchCfg& L, const ApplyChain& A, cudaStream_t st) {
-    if (A.count == 0 || A.ntiles == 0) return cudaSuccess;
-    // (pixel bytes, residual sample bytes) as in launch_gather_scatter; 0: no residual pair, the plain sweep
-    const uint32_t key = A.pix_bytes * 4u + (A.residual ? A.sample_bytes : 0u);
-    if (!(key == 1u * 4 || key == 2u * 4 || key == 3u * 4 || key == 6u * 4 || key == 1u * 4 + 1 || key == 3u * 4 + 1 ||
-          key == 2u * 4 + 2 || key == 6u * 4 + 2))
-        return cudaErrorInvalidValue;
-    k_tile_count<<<dim3((A.ntiles + 7u) / 8u, A.count), 256, 0, st>>>(A);
-    k_tile_scan<<<A.count, 1024, 0, st>>>(A);
-    L.launches += 2;
+// (pixel bytes, residual sample bytes) as in launch_gather_scatter; 0: no residual pair, the plain sweep
+static bool apply_key_ok(uint32_t key) {
+    return key == 1u * 4 || key == 2u * 4 || key == 3u * 4 || key == 6u * 4 || key == 1u * 4 + 1 || key == 3u * 4 + 1 ||
+           key == 2u * 4 + 2 || key == 6u * 4 + 2;
+}
+static cudaError_t launch_sweep(LaunchCfg& L, const ApplyChain& A, uint32_t key, cudaStream_t st) {
     switch (key) {
     case 1u * 4: return launch_apply_sweep_t<1, 0>(L, A, st);
     case 2u * 4: return launch_apply_sweep_t<2, 0>(L, A, st);
@@ -443,6 +452,68 @@ cudaError_t launch_apply_chain(LaunchCfg& L, const ApplyChain& A, cudaStream_t s
     case 2u * 4 + 2: return launch_apply_sweep_t<2, 2>(L, A, st);
     default: return launch_apply_sweep_t<6, 2>(L, A, st);
     }
+}
+static void launch_tile_prefix(LaunchCfg& L, const ApplyChain& A, cudaStream_t st) {
+    k_tile_count<<<dim3((A.ntiles + 7u) / 8u, A.count), 256, 0, st>>>(A);
+    k_tile_scan<<<A.count, 1024, 0, st>>>(A);
+    L.launches += 2;
+}
+cudaError_t launch_apply_chain(LaunchCfg& L, const ApplyChain& A, cudaStream_t st) {
+    if (A.count == 0 || A.ntiles == 0) return cudaSuccess;
+    const uint32_t key = A.pix_bytes * 4u + (A.residual ? A.sample_bytes : 0u);
+    if (!apply_key_ok(key)) return cudaErrorInvalidValue;
+    launch_tile_prefix(L, A, st);
+    return launch_sweep(L, A, key, st);
+}
+cudaError_t launch_apply_chain_motion(LaunchCfg& L, const ApplyChain& A, const uint8_t* h_modes, const int8_t* d_fields, uint32_t H,
+                                     uint32_t W, uint32_t* d_run_bad, cudaStream_t st) {
+    if (A.count == 0 || A.ntiles == 0) return cudaSuccess;
+    const uint32_t mkey = A.pix_bytes * 4u + A.sample_bytes;           // the residual kinds of launch_gather_scatter
+    if (!A.residual || !d_fields || !apply_key_ok(mkey) || mkey == A.pix_bytes * 4u) return cudaErrorInvalidValue;
+    launch_tile_prefix(L, A, st);
+    for (uint32_t t = 0; t < A.count;) {
+        if (h_modes[t] == 2) {
+            uint32_t* next_bad = t + 1u < A.count && h_modes[t + 1u] != 2 ? d_run_bad + t + 1u : nullptr;
+            switch (mkey) {
+            case 1u * 4 + 1: k_apply_motion<1, 1><<<A.ntiles, AP_THREADS, 0, st>>>(A, t, d_fields, H, W, next_bad); break;
+            case 3u * 4 + 1: k_apply_motion<3, 1><<<A.ntiles, AP_THREADS, 0, st>>>(A, t, d_fields, H, W, next_bad); break;
+            case 2u * 4 + 2: k_apply_motion<2, 2><<<A.ntiles, AP_THREADS, 0, st>>>(A, t, d_fields, H, W, next_bad); break;
+            default: k_apply_motion<6, 2><<<A.ntiles, AP_THREADS, 0, st>>>(A, t, d_fields, H, W, next_bad); break;
+            }
+            if (cudaError_t e = counted(L)) return e;
+            t++;
+            continue;
+        }
+        // a run of plain / residual pairs [t, t1) is swept as a chain of its own; a run after a motion pair checks the first failing
+        // pair counted from its start, which that motion kernel stored
+        uint32_t t1 = t;
+        bool any_residual = false;
+        for (; t1 < A.count && h_modes[t1] != 2; t1++) any_residual |= h_modes[t1] != 0;
+        ApplyChain R = A;
+        R.masks = A.masks + (size_t)t * A.mask_stride_w;
+        R.base = A.base + t >= A.max_frames ? A.base + t - A.max_frames : A.base + t;
+        R.count = t1 - t;
+        R.value_off = A.value_off + t;
+        R.residual = any_residual ? A.residual + t : nullptr;
+        R.tile_pfx = A.tile_pfx + (size_t)t * A.ntiles;
+        R.first_bad = t == 0 ? A.first_bad : d_run_bad + t;
+        if (cudaError_t e = launch_sweep(L, R, A.pix_bytes * 4u + (any_residual ? A.sample_bytes : 0u), st)) return e;
+        t = t1;
+    }
+    return cudaSuccess;
+}
+cudaError_t launch_motion_search(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t H, uint32_t W, uint32_t pix_bytes, uint32_t sample_bytes,
+                                 int8_t* d_fields, cudaStream_t st) {
+    if (F <= 0 || H == 0 || W == 0) return cudaSuccess;
+    const dim3 grid(mv_blocks(H, W), (unsigned)F);
+    switch (pix_bytes * 4u + sample_bytes) {
+    case 1u * 4 + 1: k_motion_search<1, 1><<<grid, MV_THREADS, 0, st>>>(d_pairs, H, W, d_fields); break;
+    case 3u * 4 + 1: k_motion_search<3, 1><<<grid, MV_THREADS, 0, st>>>(d_pairs, H, W, d_fields); break;
+    case 2u * 4 + 2: k_motion_search<2, 2><<<grid, MV_THREADS, 0, st>>>(d_pairs, H, W, d_fields); break;
+    case 6u * 4 + 2: k_motion_search<6, 2><<<grid, MV_THREADS, 0, st>>>(d_pairs, H, W, d_fields); break;
+    default: return cudaErrorInvalidValue;
+    }
+    return counted(L);
 }
 cudaError_t launch_median5(LaunchCfg& L, const void* d_in, uint32_t pix_stride, uint32_t H, uint32_t W, int sample_bytes, void* d_out,
                            cudaStream_t st) {

@@ -44,7 +44,16 @@ struct GatherJob {
     uint8_t* out_frame;       // scatter: destination frame (already holds the base frame)
     uint32_t npix;
     uint32_t pix_bytes;
+    uint32_t width;           // motion residual gather: frame width (the height is npix / width)
+    const int8_t* field;      // motion residual gather: the pair's (dx, dy) per 16 x 16 block, raster order; otherwise unused
 };
+
+// Block motion (rbf_motion.cuh): 16 x 16 px blocks in raster order, one (dx, dy) int8 pair per block, |dx|, |dy| <= 16.
+// pred(y, x) = prev(clamp(y + dy, 0, H - 1), clamp(x + dx, 0, W - 1)) with the vector of the block holding (y, x).
+static constexpr int MV_BLOCK = 16;
+static constexpr int MV_RANGE = 16;
+__host__ __device__ __forceinline__ uint32_t mv_blocks_x(uint32_t W) { return (W + MV_BLOCK - 1u) / MV_BLOCK; }
+__host__ __device__ __forceinline__ uint32_t mv_blocks(uint32_t H, uint32_t W) { return mv_blocks_x(W) * ((H + MV_BLOCK - 1u) / MV_BLOCK); }
 
 
 // K4c (rbf_k4c_apply.cuh): a chain of decoded masks applied to one base frame, frames base+1 .. base+count
@@ -123,7 +132,11 @@ uint32_t gather_chunks(uint32_t npix);
 // resid_sample_bytes: 0 gathers the current frame's samples; 1 or 2 gathers curr - prev per sample of that width (gather only,
 // pix_bytes / resid_sample_bytes channels of 1 or 3)
 cudaError_t launch_gather_scatter(LaunchCfg& L, const GatherJob* d_jobs, int F, int scatter, uint32_t npix, uint32_t pix_bytes,
-                                  uint32_t* d_counts, uint32_t* d_totals, cudaStream_t st, uint32_t resid_sample_bytes = 0);
+                                  uint32_t* d_counts, uint32_t* d_totals, cudaStream_t st, uint32_t resid_sample_bytes = 0,
+                                  bool motion = false);
+// block motion search of F pairs (pairs[f].prev -> pairs[f].curr): d_fields + f * mv_blocks(H, W) * 2 receives the pair's vectors
+cudaError_t launch_motion_search(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t H, uint32_t W, uint32_t pix_bytes, uint32_t sample_bytes,
+                                 int8_t* d_fields, cudaStream_t st);
 // decode side of a group (rbf_k4c_apply.cuh): masks of the raw-passthrough jobs (l == 0) from their bitmap slots; set bits per mask
 cudaError_t launch_raw_masks(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t npix, cudaStream_t st);
 cudaError_t launch_mask_popcount(LaunchCfg& L, const uint32_t* d_masks, size_t stride_w, uint32_t npix, int F, uint32_t* d_out,
@@ -131,6 +144,12 @@ cudaError_t launch_mask_popcount(LaunchCfg& L, const uint32_t* d_masks, size_t s
 // K4c: tile counts, tile scan (+ the ivc:882 check) and the chained sweep; *A.first_bad must hold UINT32_MAX before the launch.
 // A.residual == NULL runs the plain sweep, which has no residual branch at all
 cudaError_t launch_apply_chain(LaunchCfg& L, const ApplyChain& A, cudaStream_t st);
+// K4c with motion pairs: h_modes[t] (host) is 0 plain, 1 residual, 2 motion-compensated residual; A.residual holds the same modes on
+// the device, d_fields the [count][mv_blocks(H, W)][2] block vectors.  One tile count + scan for the whole chain, then one
+// k_apply_sweep per run of plain / residual pairs and one k_apply_motion per motion pair, in order on `st`.  d_run_bad: count words
+// of scratch (a run's first failing pair, counted from the run's start).
+cudaError_t launch_apply_chain_motion(LaunchCfg& L, const ApplyChain& A, const uint8_t* h_modes, const int8_t* d_fields, uint32_t H,
+                                     uint32_t W, uint32_t* d_run_bad, cudaStream_t st);
 cudaError_t launch_median5(LaunchCfg& L, const void* d_in, uint32_t pix_stride, uint32_t H, uint32_t W, int sample_bytes, void* d_out,
                            cudaStream_t st);
 cudaError_t launch_bitrev(LaunchCfg& L, uint32_t* d_words, size_t nwords, cudaStream_t st);

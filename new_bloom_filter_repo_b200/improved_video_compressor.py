@@ -344,24 +344,26 @@ class VideoFrameCompressor:
 _INTER_TAG_V1 = b"\xff\xff\xff\xffRBF1"   # round-1 layout: raw-passthrough masks stored as plain np.packbits bytes
 _INTER_TAG = b"\xff\xff\xff\xffRBF2"      # current: raw-passthrough masks zlib-compressed (a static scene costs ~1 KB, not n/8 B)
 _INTER_TAG_V3 = b"\xff\xff\xff\xffRBF3"   # value_coding "adaptive": RBF2 plus a vmode byte after the raw flag (0 values, 1 residuals)
+_INTER_TAG_V4 = b"\xff\xff\xff\xffRBF4"   # value_coding "motion": RBF3 whose vmode may be 2, followed by <I length + zlib(motion field)
 # none can be a FixedVideoCompressor payload (height 0xFFFFFFFF).  NOTE: inter payloads exist only in this implementation --
 # the reference's decoder knows keyframes only (ivc:1124); files written with keyframe_interval=1 are interchangeable.
-_INTER_TAGS = (_INTER_TAG, _INTER_TAG_V1, _INTER_TAG_V3)
+_INTER_TAGS = (_INTER_TAG, _INTER_TAG_V1, _INTER_TAG_V3, _INTER_TAG_V4)
 
 
 class _InterPayload:
     """The fields of one inter-frame payload (ImprovedVideoCompressor._parse_inter); the byte fields are views of the payload.
-    vmode 1: the value stream holds residuals (curr - prev) mod 2^(8 isz) per sample instead of the current samples."""
+    vmode 1: the value stream holds residuals (curr - prev) mod 2^(8 isz) per sample instead of the current samples; vmode 2: residuals
+    against the motion-compensated previous frame, whose block vectors `fz` holds (zlib)."""
     __slots__ = ("v1", "h", "w", "isz", "ch", "raw", "vmode", "k", "l", "wlen", "ones", "mask_bytes", "witness_bytes", "vcount",
-                 "vz")
+                 "vz", "fz")
 
 
 class _InterJob:
     """An inter frame on its way through decompress_video: the parsed payload (or its parse error) and its inflates."""
-    __slots__ = ("p", "err", "values", "mask", "values_arr", "mask_arr", "l", "wlen")
+    __slots__ = ("p", "err", "values", "mask", "field", "values_arr", "mask_arr", "field_arr", "l", "wlen")
 
     def __init__(self):
-        self.p = self.err = self.values = self.mask = self.values_arr = self.mask_arr = None
+        self.p = self.err = self.values = self.mask = self.field = self.values_arr = self.mask_arr = self.field_arr = None
         self.l = self.wlen = 0
 
 
@@ -385,6 +387,10 @@ class ImprovedVideoCompressor:
       "adaptive"  per inter frame, whichever zlib stream is shorter: those samples, or the residuals (curr - prev) mod 2^bits per
                   sample; a tie goes to the samples ('RBF3' payloads, whose vmode byte says which).  The decoder adds residuals to
                   the previous frame, which equals the encoder's original previous frame in both inter_frame_modes.
+      "motion"    per inter frame, the cheapest of those two and the residuals against the motion-compensated previous frame: one
+                  (dx, dy) in [-16, 16]^2 per 16 x 16 block, found by a full SAD search on the GPU, predicts each pixel from
+                  prev(clamp(y + dy), clamp(x + dx)).  That option costs its stream plus 4 + the zlib'd field; the strict minimum wins and a
+                  tie goes to the lower vmode ('RBF4' payloads: 'RBF3' plus the field when vmode is 2).
     """
 
     def __init__(self, noise_tolerance: float = 10.0, keyframe_interval: int = 30, min_diff_threshold: float = 3.0,
@@ -422,21 +428,43 @@ class ImprovedVideoCompressor:
         return (dz, 1) if len(dz) < len(vz) else (vz, 0)
 
     @staticmethod
-    def _inter_payload(shape, itemsize, ch, r, bm_row, wt_row, mask_row, values, resids=None) -> bytes:
-        """Assemble one inter-frame payload (runs in a worker thread; the zlib calls release the GIL).  With `resids` (adaptive
-        value coding) both value streams are compressed and the shorter one is kept."""
-        vz, vmode = ImprovedVideoCompressor._choose_values(zlib.compress(values.tobytes(), 9),
-                                                           None if resids is None else zlib.compress(resids.tobytes(), 9))
-        rz = zlib.compress(ImprovedVideoCompressor._raw_mask_bits(shape, mask_row), 9) if r.raw else None
-        return ImprovedVideoCompressor._inter_layout(shape, itemsize, ch, r, bm_row, wt_row, rz, vz, values.size, vmode)
+    def _choose_motion(vz: bytes, dz: bytes, mz: bytes, fz: bytes):
+        """-> (value stream, vmode, zlib'd field or None) of value_coding "motion": the cheapest of the values (len(vz)), the residuals
+        (len(dz)) and the motion residuals with their field (len(mz) + 4 + len(fz)); a tie goes to the lower vmode."""
+        costs = (len(vz), len(dz), len(mz) + 4 + len(fz))
+        vmode = costs.index(min(costs))
+        return (vz, dz, mz)[vmode], vmode, fz if vmode == 2 else None
 
     @staticmethod
-    def _inter_layout(shape, itemsize, ch, r, bm_row, wt_row, rz, vz, vcount, vmode=None) -> bytes:
+    def _inter_payload(shape, itemsize, ch, r, bm_row, wt_row, mask_row, values, resids=None, mresids=None, field=None) -> bytes:
+        """Assemble one inter-frame payload (runs in a worker thread; the zlib calls release the GIL).  With `resids` (adaptive
+        value coding) both value streams are compressed and the shorter one is kept; with `mresids` and `field` as well (motion value
+        coding) the three options are costed by _choose_motion."""
+        vz = zlib.compress(values.tobytes(), 9)
+        dz = None if resids is None else zlib.compress(resids.tobytes(), 9)
+        fz = None
+        if mresids is not None:
+            vz, vmode, fz = ImprovedVideoCompressor._choose_motion(vz, dz, zlib.compress(mresids.tobytes(), 9),
+                                                                   zlib.compress(field.tobytes(), 9))
+        else:
+            vz, vmode = ImprovedVideoCompressor._choose_values(vz, dz)
+        rz = zlib.compress(ImprovedVideoCompressor._raw_mask_bits(shape, mask_row), 9) if r.raw else None
+        return ImprovedVideoCompressor._inter_layout(shape, itemsize, ch, r, bm_row, wt_row, rz, vz, values.size, vmode, fz,
+                                                     mresids is not None)
+
+    @staticmethod
+    def _inter_layout(shape, itemsize, ch, r, bm_row, wt_row, rz, vz, vcount, vmode=None, fz=None, v4=False) -> bytes:
         """The inter-frame byte layout around the compressed raw mask `rz` (raw pairs only) and changed values `vz`.  vmode None
-        writes 'RBF2'; 0 (values) or 1 (residuals) writes 'RBF3', which carries it in one byte after the raw flag."""
-        hdr = (_INTER_TAG if vmode is None else _INTER_TAG_V3) + struct.pack("<IIIBB", shape[0], shape[1], itemsize, ch, 1 if r.raw else 0)
+        writes 'RBF2'; 0 (values) or 1 (residuals) writes 'RBF3', which carries it in one byte after the raw flag.  v4 writes 'RBF4',
+        byte for byte the 'RBF3' layout, where vmode 2 (motion residuals) is followed by <I len(fz) and fz, the zlib'd motion field."""
+        if vmode == 2 and (not v4 or fz is None):
+            raise ValueError("vmode 2 is an 'RBF4' payload with a motion field")
+        tag = _INTER_TAG if vmode is None else (_INTER_TAG_V4 if v4 else _INTER_TAG_V3)
+        hdr = tag + struct.pack("<IIIBB", shape[0], shape[1], itemsize, ch, 1 if r.raw else 0)
         if vmode is not None:
             hdr += struct.pack("<B", vmode)
+        if vmode == 2:
+            hdr += struct.pack("<I", len(fz)) + fz
         body = struct.pack("<dIIQ", r.k, r.l, r.wlen, r.ones)
         if r.raw:
             body += struct.pack("<I", len(rz)) + rz + struct.pack("<I", 0)
@@ -458,11 +486,19 @@ class ImprovedVideoCompressor:
         p.h, p.w, p.isz, p.ch, p.raw = struct.unpack_from("<IIIBB", payload, pos)
         pos += struct.calcsize("<IIIBB")
         p.vmode = 0
-        if tag == _INTER_TAG_V3:
+        p.fz = None
+        if tag in (_INTER_TAG_V3, _INTER_TAG_V4):
             (p.vmode,) = struct.unpack_from("<B", payload, pos)
             pos += 1
-            if p.vmode not in (0, 1):
+            if tag == _INTER_TAG_V3 and p.vmode not in (0, 1):
                 raise ValueError(f"corrupt inter frame: value coding {p.vmode} is neither 0 (values) nor 1 (residuals)")
+            if p.vmode not in (0, 1, 2):
+                raise ValueError(f"corrupt inter frame: value coding {p.vmode} is not 0 (values), 1 (residuals) or 2 (motion residuals)")
+            if p.vmode == 2:
+                (fl,) = struct.unpack_from("<I", payload, pos); pos += 4
+                if pos + fl > len(payload):
+                    raise ValueError(f"corrupt inter frame: a motion field of {fl} bytes runs past the payload")
+                p.fz = mv[pos:pos + fl]; pos += fl
         p.k, p.l, p.wlen, p.ones = struct.unpack_from("<dIIQ", payload, pos)
         pos += struct.calcsize("<dIIQ")
         (bl,) = struct.unpack_from("<I", payload, pos); pos += 4
@@ -496,7 +532,8 @@ class ImprovedVideoCompressor:
                     self._gpu_inter_payloads(st, shape, dtype.itemsize, ch, idxs, res, bms, wts, masks, out, pool)
                     continue
                 gathered = st.gather_changed(len(idxs))            # N1: changed values of every pair, one launch, one copy
-                resids = self._with_residuals(st, st.gather_changed, len(idxs)) if self.value_coding == "adaptive" else None
+                resids = self._with_residuals(st, st.gather_changed, len(idxs)) if self.value_coding != "plain" else None
+                fields, mres = self._with_motion(st, st.gather_changed, len(idxs)) if self.value_coding == "motion" else (None, None)
                 for j, i in enumerate(idxs):
                     r = res[j]
                     if r.resid and self.inter_frame_mode != "lossless":
@@ -504,7 +541,8 @@ class ImprovedVideoCompressor:
                         continue
                     out[i] = pool.submit(self._inter_payload, shape, dtype.itemsize, ch, r, bms[j], wts[j],
                                          masks[j] if (masks is not None and r.raw) else None, gathered[j],
-                                         None if resids is None else resids[j])
+                                         None if resids is None else resids[j], None if mres is None else mres[j],
+                                         None if fields is None else fields[j])
         finally:
             st.close()
         return out
@@ -518,22 +556,41 @@ class ImprovedVideoCompressor:
         finally:
             st.set_option("value_mode", 0)
 
+    @staticmethod
+    def _with_motion(st: FrameStream, fn, pairs: int):
+        """(the block motion fields of the encoded pairs, fn(pairs) with the stream's gathers returning residuals against the
+        motion-compensated previous frames (motion_values 1))."""
+        fields = st.motion_search(pairs)
+        st.set_option("motion_values", 1)
+        try:
+            return fields, fn(pairs)
+        finally:
+            st.set_option("motion_values", 0)
+
     def _gpu_inter_payloads(self, st, shape, itemsize, ch, idxs, res, bms, wts, masks, out, pool) -> None:
-        """entropy_coder "gpu": changed values (and, adaptive, their residuals) deflated where they were gathered (N1 + N4), raw masks
-        in one batch."""
-        vzs = st.zlib_changed(len(idxs))
-        dzs = self._with_residuals(st, st.zlib_changed, len(idxs)) if self.value_coding == "adaptive" else [None] * len(idxs)
-        voffs = st.changed_offsets(len(idxs))
+        """entropy_coder "gpu": changed values (and, adaptive or motion, their residuals) deflated where they were gathered (N1 + N4),
+        raw masks and motion fields in one batch each."""
+        n = len(idxs)
+        vzs = st.zlib_changed(n)
+        dzs = self._with_residuals(st, st.zlib_changed, n) if self.value_coding != "plain" else [None] * n
+        fields, mzs = self._with_motion(st, st.zlib_changed, n) if self.value_coding == "motion" else (None, None)
+        voffs = st.changed_offsets(n)
         keep = [j for j, i in enumerate(idxs) if not (res[j].resid and self.inter_frame_mode != "lossless")]
         raw_js = [j for j in keep if res[j].raw]
         rzs = dict(zip(raw_js, deflate.compress_many([self._raw_mask_bits(shape, masks[j]) for j in raw_js])))
+        fzs = dict(zip(keep, deflate.compress_many([fields[j].tobytes() for j in keep]))) if fields is not None else {}
         for j, i in enumerate(idxs):
             if j not in keep:
                 out[i] = None                                      # not exactly representable: keyframe instead
                 continue
             vcount = int(voffs[j + 1] - voffs[j]) // itemsize
-            vz, vmode = self._choose_values(vzs[j], dzs[j])
-            out[i] = pool.submit(self._inter_layout, shape, itemsize, ch, res[j], bms[j], wts[j], rzs.get(j), vz, vcount, vmode)
+            fz = None
+            if mzs is not None:
+                vz, vmode, fz = self._choose_motion(vzs[j], dzs[j], mzs[j], fzs[j])
+            else:
+                vz, vmode = self._choose_values(vzs[j], dzs[j])
+            out[i] = pool.submit(self._inter_layout, shape, itemsize, ch, res[j], bms[j], wts[j], rzs.get(j), vz, vcount, vmode, fz,
+                                 mzs is not None)
 
     def _keyframe_job(self, frame, pool):
         """Callable returning the keyframe payload of `frame`: zlib level 9 in the pool, or coded on the GPU now."""
@@ -545,8 +602,8 @@ class ImprovedVideoCompressor:
     def compress_video(self, frames: List[np.ndarray], output_path: str = None, input_color_space: str = "BGR") -> Dict:
         if self.entropy_coder not in ("zlib", "gpu"):
             raise ValueError(f"entropy_coder must be 'zlib' or 'gpu', not {self.entropy_coder!r}")
-        if self.value_coding not in ("plain", "adaptive"):
-            raise ValueError(f"value_coding must be 'plain' or 'adaptive', not {self.value_coding!r}")
+        if self.value_coding not in ("plain", "adaptive", "motion"):
+            raise ValueError(f"value_coding must be 'plain', 'adaptive' or 'motion', not {self.value_coding!r}")
         if not frames:
             raise ValueError("No frames provided for compression")                 # ivc:372-373
         start_time = time.time()
@@ -613,6 +670,8 @@ class ImprovedVideoCompressor:
             job.err = e
             return job
         job.values = pool.submit(zlib.decompress, job.p.vz)
+        if job.p.vmode == 2:
+            job.field = pool.submit(zlib.decompress, job.p.fz)
         if job.p.raw and not job.p.v1:
             job.mask = pool.submit(zlib.decompress, job.p.mask_bytes)
         return job
@@ -631,6 +690,13 @@ class ImprovedVideoCompressor:
             raise ValueError(f"inter frame {exp_shape}/{dtype} does not match the previous frame {pdata.shape}/{pdata.dtype}")
         if job.values_arr.size != p.ones * p.ch:
             raise ValueError(f"corrupt inter frame: {job.values_arr.size} changed values for {p.ones} changed pixels x {p.ch} channels")
+        if p.vmode == 2:
+            nfield = 2 * ((p.h + 15) // 16) * ((p.w + 15) // 16)
+            job.field_arr = np.frombuffer(job.field.result(), dtype=np.int8)
+            if job.field_arr.size != nfield:
+                raise ValueError(f"corrupt inter frame: a motion field of {job.field_arr.size} bytes for {nfield // 2} blocks")
+            if job.field_arr.size and np.abs(job.field_arr.astype(np.int16)).max() > 16:
+                raise ValueError("corrupt inter frame: a motion vector component outside [-16, 16]")
         if p.raw:
             job.mask_arr = np.frombuffer(p.mask_bytes if p.v1 else job.mask.result(), dtype=np.uint8)
             if job.mask_arr.size < (p.h * p.w + 7) // 8:
@@ -646,7 +712,8 @@ class ImprovedVideoCompressor:
     @staticmethod
     def _decode_group(st: FrameStream, base: int, group: List["_InterJob"]) -> np.ndarray:
         """Frames base+1 .. base+len(group) of `st` (slots modulo st.max_frames) from frame `base` and the group's payloads: one
-        decode_masks, one apply_chain and one download_batch.  Raises the first bad frame's error."""
+        decode_masks, one apply_chain (value modes and motion fields included) and one download_batch.  Raises the first bad frame's
+        error."""
         m, n = len(group), st.npix
         raws = [bool(j.p.raw) for j in group]
         nbs = [(n + 7) // 8 if r else (j.l + 7) // 8 for j, r in zip(group, raws)]
@@ -666,7 +733,8 @@ class ImprovedVideoCompressor:
                 raise IndexError("list index out of range")
             if ones[i] != j.p.ones:                          # the reference would silently return the base frame (ivc:882)
                 raise ValueError(f"corrupt inter frame: the decoded mask selects {int(ones[i])} pixels, the payload announces {j.p.ones}")
-        applied = st.apply_chain(base, [j.values_arr for j in group], residual=[j.p.vmode for j in group])
+        applied = st.apply_chain(base, [j.values_arr for j in group], residual=[j.p.vmode for j in group],
+                                 motion=[j.field_arr for j in group])
         if not np.array_equal(applied, ones):
             raise ValueError(f"corrupt inter frame: {applied.tolist()} pixels applied, {ones.tolist()} expected")
         return st.download_batch((base + 1) % st.max_frames, m)

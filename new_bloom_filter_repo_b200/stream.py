@@ -37,6 +37,7 @@ class FrameStream:
         self.max_frames = int(max_frames)
         self.max_pairs = int(max_pairs if max_pairs is not None else max(1, max_frames - 1))
         self.npix = self.H * self.W
+        self.mv_shape = ((self.H + 15) // 16, (self.W + 15) // 16)      # 16 x 16 motion blocks (rows, columns)
         self._h = C.c_void_p()
         _cabi.check(_cabi.lib().rbf_stream_create(_cabi.ctx(), self.H, self.W, self.C, dt.itemsize, self.max_frames,
                                                   self.max_pairs, C.byref(self._h)), _cabi.ctx())
@@ -48,7 +49,8 @@ class FrameStream:
 
     def set_option(self, key: str, value: int) -> None:
         """Per-stream option of the C ABI (rbf_stream_set_option): k1_only, mask_mode, gray_mode, value_mode (0: gather_changed and
-        zlib_changed return the current samples; 1: residuals (curr - prev) mod 2^bits per sample)."""
+        zlib_changed return the current samples; 1: residuals (curr - prev) mod 2^bits per sample), motion_values (1: residuals
+        against the motion-compensated previous frame of the last motion_search)."""
         _cabi.check(_cabi.lib().rbf_stream_set_option(self._h, key.encode(), int(value)), _cabi.ctx())
         if key == "k1_only":
             self.k1_only = bool(value)
@@ -164,6 +166,15 @@ class FrameStream:
         _cabi.check(_cabi.lib().rbf_stream_zlib_changed(self._h, n, _cabi.ptr(out), cap, _cabi.ptr(offs)), _cabi.ctx())
         return [out[int(offs[i]):int(offs[i + 1])].tobytes() for i in range(n)]
 
+    def motion_search(self, pairs: Optional[int] = None) -> np.ndarray:
+        """Block motion of every encoded pair, prev -> curr: int8 [pairs, by, bx, 2] of (dx, dy) per 16 x 16 block in [-16, 16], the
+        vector minimising the SAD of curr against prev(clamp(y + dy), clamp(x + dx)); ties go to the smaller |dx| + |dy|, then dy,
+        then dx.  The fields stay in the stream for gathers with motion_values 1 until the next encode."""
+        n = self.pairs if pairs is None else int(pairs)
+        out = np.zeros((n,) + self.mv_shape + (2,), dtype=np.int8)
+        _cabi.check(_cabi.lib().rbf_stream_motion_search(self._h, n, _cabi.ptr(out)), _cabi.ctx())
+        return out
+
     def apply_diff(self, base_frame: int, out_frame: int, mask: np.ndarray, values: np.ndarray) -> int:
         """store[out_frame] = store[base_frame] with masked pixels replaced by `values` (ivc:849-909); returns pixels applied."""
         mk = np.packbits(np.ascontiguousarray(mask, dtype=np.uint8).reshape(-1), bitorder="little")
@@ -202,11 +213,16 @@ class FrameStream:
         self.pairs = 0
         return consumed, ones
 
-    def apply_chain(self, base_frame: int, values: Sequence[np.ndarray], residual: Optional[Sequence[int]] = None) -> np.ndarray:
+    def apply_chain(self, base_frame: int, values: Sequence[np.ndarray], residual: Optional[Sequence[int]] = None,
+                    motion: Optional[Sequence[Optional[np.ndarray]]] = None) -> np.ndarray:
         """Frame base_frame+1+i = frame base_frame+i with mask slot i applied, values[i] replacing its set pixels in rank order
         (ivc:849-909), for i < len(values); slots are taken modulo max_frames.  residual[i] = 1 adds values[i] to the set pixels
-        per sample (mod 2^bits) instead: the residuals a value_mode=1 gather returns.  -> uint64[count] pixels applied per pair: 0
-        from the first pair whose value count does not match its mask (ivc:882), whose frame and every later one are not written."""
+        per sample (mod 2^bits) instead: the residuals a value_mode=1 gather returns.  residual[i] = 2 adds them to the motion-compensated
+        prediction from frame base_frame+i under motion[i], pair i's int8 field of motion_search's shape [by, bx, 2] (motion[j] is
+        ignored, and may be None, for the other pairs): the residuals a motion_values=1 gather returns.  A mode-2 pair whose motion[i]
+        is None raises ValueError; without `motion` the flags go to rbf_stream_apply_chain_modes, which refuses 2.  -> uint64[count] pixels applied
+        per pair: 0 from the first pair whose value count does not match its mask (ivc:882), whose frame and every later one are not
+        written."""
         parts = [memoryview(np.ascontiguousarray(v)).cast("B") for v in values]
         offs = np.zeros(len(parts) + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([p.nbytes for p in parts])
@@ -217,6 +233,20 @@ class FrameStream:
             flags = np.ascontiguousarray(np.asarray(residual, dtype=np.uint8))
             if flags.shape != (len(parts),):
                 raise ValueError("one residual flag per pair")
+        if motion is not None and flags is not None and (flags == 2).any():
+            fields = np.zeros((len(parts),) + self.mv_shape + (2,), dtype=np.int8)
+            for i in np.flatnonzero(flags == 2):
+                f = motion[i] if i < len(motion) else None
+                if f is None:
+                    raise ValueError(f"pair {i} is a motion pair without a motion field")
+                f = np.asarray(f)
+                if f.dtype != np.int8 or f.size != fields[i].size:
+                    raise ValueError(f"pair {i}: a motion field is {fields[i].size} int8 values, not {f.size} {f.dtype}")
+                fields[i] = f.reshape(fields[i].shape)
+            _cabi.check(_cabi.lib().rbf_stream_apply_chain_motion(self._h, int(base_frame), len(parts), _cabi.ptr(buf) if buf.size else None,
+                                                                  _cabi.ptr(offs), _cabi.ptr(flags), _cabi.ptr(fields), _cabi.ptr(applied)),
+                        _cabi.ctx())
+            return applied
         _cabi.check(_cabi.lib().rbf_stream_apply_chain_modes(self._h, int(base_frame), len(parts), _cabi.ptr(buf) if buf.size else None,
                                                              _cabi.ptr(offs), _cabi.ptr(flags) if flags is not None else None,
                                                              _cabi.ptr(applied)), _cabi.ctx())
