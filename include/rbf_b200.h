@@ -119,7 +119,9 @@ int rbf_filter_add_strings(rbf_filter* f, const uint8_t* blob, const uint64_t* o
 int rbf_filter_check_strings(rbf_filter* f, const uint8_t* blob, const uint64_t* offsets, uint32_t count, int standard_k,
                              uint8_t* out01);
 int rbf_filter_get_bits(rbf_filter* f, uint8_t* unpacked_out);        /* size bytes of 0/1 */
-int rbf_filter_set_bits(rbf_filter* f, const uint8_t* unpacked_in);   /* `bloom_filter.bit_array = bitmap`, ivc:290 */
+int rbf_filter_set_bits(rbf_filter* f, const uint8_t* unpacked_in);   /* `bloom_filter.bit_array = bitmap`, ivc:290: replaces every
+                                                                          bit; any non-zero byte is set, as `bit_array[idx] == 0`
+                                                                          tests it (ivc:129,135), so get_bits then reads it as 1 */
 
 /* ------------------------------------------------------------------ mask coder (drop-in BloomFilterCompressor)
  * compress (ivc:198-266): mask_unpacked[n] (0/1) -> info, bitmap_unpacked_out[l], witness_unpacked_out[wlen].
@@ -129,6 +131,8 @@ int rbf_compress_mask(rbf_ctx* ctx, const uint8_t* mask_unpacked, uint64_t n, co
                       uint64_t l_override, rbf_mask_info* info, uint8_t* bitmap_unpacked_out,
                       uint8_t* witness_unpacked_out);
 /* decompress (ivc:268-307): bitmap_unpacked[l], witness_unpacked[wlen], n, k -> mask_unpacked_out[n].
+ * Any non-zero bitmap byte is a set bit, as the reference's filter reads the bitmap it is given (ivc:290, ivc:129,135);
+ * a witness byte is a bit only when it is 1.
  * *consumed = number of positions that passed the Bloom test (the reference raises IndexError when > wlen). */
 int rbf_decompress_mask(rbf_ctx* ctx, const uint8_t* bitmap_unpacked, uint64_t l, const uint8_t* witness_unpacked,
                         uint64_t wlen, uint64_t n, double k, const rbf_seeds* seeds, uint8_t* mask_unpacked_out,

@@ -447,7 +447,7 @@ extern "C" int rbf_filter_set_bits(rbf_filter* f, const uint8_t* in) {
     if ((rc = scratch_get(c, kScrBytes, f->size, &d_bytes))) return rc;
     CK(c, cudaMemcpyAsync(d_bytes, in, f->size, cudaMemcpyHostToDevice, c->st)); c->h2d += f->size;
     CK(c, cudaMemsetAsync(f->d_bits, 0, f->words * 4, c->st));
-    CK(c, launch_pack_bytes(c->L, (const uint8_t*)d_bytes, f->d_bits, f->size, c->st));
+    CK(c, launch_pack_bytes(c->L, (const uint8_t*)d_bytes, f->d_bits, f->size, 1, c->st));     // any non-zero byte is set (ivc:129,135)
     CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
 }
@@ -501,7 +501,7 @@ extern "C" int rbf_compress_mask(rbf_ctx* c, const uint8_t* mask, uint64_t n, co
     CK(c, cudaMemcpyAsync(d_bytes, mask, n, cudaMemcpyHostToDevice, c->st)); c->h2d += n;
     CK(c, cudaMemsetAsync(d_mask, 0, mw * 4, c->st));
     CK(c, cudaMemsetAsync(d_cnt, 0, 16, c->st));
-    CK(c, launch_pack_bytes(c->L, (const uint8_t*)d_bytes, (uint32_t*)d_mask, n, c->st));
+    CK(c, launch_pack_bytes(c->L, (const uint8_t*)d_bytes, (uint32_t*)d_mask, n, 0, c->st));    // `binary_input[i] == 1`, ivc:236
     CK(c, launch_popcount(c->L, (const uint32_t*)d_mask, (n + 31) / 32, d_cnt, c->st));
     uint32_t h_cnt[4] = {0, 0, 0, 0};
     CK(c, cudaMemcpyAsync(h_cnt, d_cnt, 16, cudaMemcpyDeviceToHost, c->st)); c->d2h += 16;
@@ -563,12 +563,12 @@ extern "C" int rbf_decompress_mask(rbf_ctx* c, const uint8_t* bitmap, uint64_t l
     CK(c, cudaMemsetAsync(d_wit, 0, ww * 4, c->st));
     CK(c, cudaMemsetAsync(d_out, 0, mw * 4, c->st));
     CK(c, cudaMemcpyAsync(d_bytes, bitmap, l, cudaMemcpyHostToDevice, c->st)); c->h2d += l;
-    CK(c, launch_pack_bytes(c->L, (const uint8_t*)d_bytes, (uint32_t*)d_bits, l, c->st));
+    CK(c, launch_pack_bytes(c->L, (const uint8_t*)d_bytes, (uint32_t*)d_bits, l, 1, c->st));     // the filter's bit array: non-zero is set
     if (wlen) {
         CK(c, cudaMemcpyAsync(d_bytes, witness, wlen, cudaMemcpyHostToDevice, c->st)); c->h2d += wlen;
         // witness values are used as bits: any non-zero byte other than 1 is not representable; the reference
         // stores whatever the list holds (ivc:303); np.unpackbits output is 0/1 (ivc:1001-1002)
-        CK(c, launch_pack_bytes(c->L, (const uint8_t*)d_bytes, (uint32_t*)d_wit, wlen, c->st));
+        CK(c, launch_pack_bytes(c->L, (const uint8_t*)d_bytes, (uint32_t*)d_wit, wlen, 0, c->st));
     }
     FrameJob J = frame_job(n, l, k, *sd, (uint32_t*)d_bits, (uint32_t*)d_wit, (uint32_t*)d_pass);
     J.out_mask = (uint32_t*)d_out;

@@ -153,13 +153,14 @@ __global__ void k_unpack_bits(const uint32_t* __restrict__ w, uint8_t* __restric
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nbits; i += (size_t)gridDim.x * blockDim.x)
         out[i] = (uint8_t)((w[i >> 5] >> (i & 31)) & 1u);
 }
-// one byte per position (== 1 is set, as `binary_input[i] == 1`, ivc:236) -> LSB-first packed words
-__global__ void k_pack_bytes(const uint8_t* __restrict__ in, uint32_t* __restrict__ w, size_t nbits) {
+// one byte per position -> LSB-first packed words.  nonzero = 0: a byte == 1 is set, as the mask test `binary_input[i] == 1`
+// (ivc:236); nonzero = 1: any non-zero byte is set, as a Bloom bit array is read (`bit_array[idx] == 0` is unset, ivc:129,135)
+__global__ void k_pack_bytes(const uint8_t* __restrict__ in, uint32_t* __restrict__ w, size_t nbits, int nonzero) {
     const size_t nwords = (nbits + 31) >> 5;
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nwords; i += (size_t)gridDim.x * blockDim.x) {
         uint32_t v = 0;
         const size_t b0 = i << 5;
-        for (uint32_t k = 0; k < 32u && b0 + k < nbits; k++) v |= (in[b0 + k] == 1 ? 1u : 0u) << k;
+        for (uint32_t k = 0; k < 32u && b0 + k < nbits; k++) v |= ((nonzero ? in[b0 + k] != 0 : in[b0 + k] == 1) ? 1u : 0u) << k;
         w[i] = v;
     }
 }

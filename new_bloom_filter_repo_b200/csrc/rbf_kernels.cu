@@ -534,9 +534,9 @@ cudaError_t launch_unpack_bits(LaunchCfg& L, const uint32_t* d_words, uint8_t* d
     k_unpack_bits<<<grid_for(nbits, 256, L.sm_count), 256, 0, st>>>(d_words, d_out, nbits);
     return counted(L);
 }
-cudaError_t launch_pack_bytes(LaunchCfg& L, const uint8_t* d_bytes, uint32_t* d_words, size_t nbits, cudaStream_t st) {
+cudaError_t launch_pack_bytes(LaunchCfg& L, const uint8_t* d_bytes, uint32_t* d_words, size_t nbits, int nonzero, cudaStream_t st) {
     if (nbits == 0) return cudaSuccess;
-    k_pack_bytes<<<grid_for((nbits + 31) / 32, 256, L.sm_count), 256, 0, st>>>(d_bytes, d_words, nbits);
+    k_pack_bytes<<<grid_for((nbits + 31) / 32, 256, L.sm_count), 256, 0, st>>>(d_bytes, d_words, nbits, nonzero);
     return counted(L);
 }
 

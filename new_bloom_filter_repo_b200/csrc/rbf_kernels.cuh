@@ -158,7 +158,8 @@ cudaError_t launch_unpack_bits_msb(LaunchCfg& L, const uint32_t* d_words, uint8_
 cudaError_t launch_popcount(LaunchCfg& L, const uint32_t* d_words, size_t nwords, uint32_t* d_out, cudaStream_t st);
 cudaError_t launch_count_diff(LaunchCfg& L, const uint32_t* a, const uint32_t* b, size_t stride_words, size_t nwords, int F,
                               uint32_t* d_out, cudaStream_t st);
-cudaError_t launch_pack_bytes(LaunchCfg& L, const uint8_t* d_bytes, uint32_t* d_words, size_t nbits, cudaStream_t st);
+// nonzero = 0: a byte == 1 is a set bit (a 0/1 mask); nonzero = 1: any non-zero byte is (a caller's Bloom bit array)
+cudaError_t launch_pack_bytes(LaunchCfg& L, const uint8_t* d_bytes, uint32_t* d_words, size_t nbits, int nonzero, cudaStream_t st);
 
 // explicit-item kernels (drop-in RationalBloomFilter.add_index/check_index, rbf add/contains)
 cudaError_t launch_items_u32(LaunchCfg& L, const FrameJob* d_job, const uint32_t* d_items, uint32_t count, uint8_t* d_result,

@@ -71,13 +71,14 @@ class RationalBloomFilter:
     @staticmethod
     def _split(indices):
         """uint32 items go to the decimal-index kernels; anything else the reference would hash as str(item) -- negative or
-        >= 2**32 integers -- goes through the string kernels, so `str(item)` semantics hold for every int."""
+        >= 2**32 integers, floats, strings, bools ("True") -- goes through the string kernels, so `str(item)` semantics hold."""
         arr = np.asarray(indices)
         if arr.dtype.kind in "iu" and arr.size and (arr.dtype.kind == "u" or int(arr.min()) >= 0) and int(arr.max()) < 2 ** 32:
             return arr.astype(np.uint32, copy=False).reshape(-1), None
         if arr.size == 0:
             return np.zeros(0, dtype=np.uint32), None
-        return None, [str(int(x)) if isinstance(x, (int, np.integer)) else str(x) for x in np.asarray(indices, dtype=object).reshape(-1)]
+        return None, [str(int(x)) if isinstance(x, (int, np.integer)) and not isinstance(x, (bool, np.bool_)) else str(x)
+                      for x in np.asarray(indices, dtype=object).reshape(-1)]
 
     def add_index(self, index: int) -> None:                  # ivc:99-114
         self.add_indices([index])

@@ -719,6 +719,33 @@ def test_index_filter_items_outside_uint32_follow_str_semantics(pkg, co):
     g = pkg.IndexRationalBloomFilter(5000, 2.6)
     g.bit_array = bits
     assert np.array_equal(g.bit_array, bits)
+    # every other item type, as an array of its own: each element hashes as str(element)
+    typed = [np.array([2 ** 32, 2 ** 33 + 5, 2 ** 40 + 9, 2 ** 64 - 1], dtype=np.uint64),
+             np.array([0, 5, 123456789, 2 ** 31, 2 ** 32 - 1], dtype=np.int64),          # no negatives: the index kernels
+             np.array([-3, 0, 42, -2 ** 40, 2 ** 40], dtype=np.int64),
+             np.array([5.0, -0.5, 1e20, 2.5e-7, 3.25]),
+             ["5", "abc", "", "-0"],
+             np.array([True, False]),
+             np.array([7, "x", 2.5, -1, 2 ** 70, True, np.uint64(2 ** 63), "7"], dtype=object)]
+    for arr in typed:
+        names = [str(x) for x in arr]
+        h =pkg.IndexRationalBloomFilter(5000, 2.6)
+        h.add_indices(arr)
+        want = np.zeros(5000, dtype=np.uint8)
+        co.filter_add_strings(want, 2.6, pkg._cabi.IVC_SEEDS, names)
+        assert np.array_equal(h.bit_array, want), names
+        assert h.check_indices(arr).all() and h.check_index(arr[0])
+        probe = np.concatenate([np.asarray(arr, dtype=object), np.array([6, "6", 6.0, False, -6, 2 ** 32 + 6], dtype=object)])
+        assert np.array_equal(h.check_indices(probe),
+                              co.filter_check_strings(want, 2.6, pkg._cabi.IVC_SEEDS, [str(x) for x in probe]).astype(bool)), names
+    assert [str(x) for x in typed[5]] == ["True", "False"] and [str(x) for x in typed[3]][0] == "5.0"
+    # "5" (string kernel) sets the bits of 5 (index kernel); 5.0 those of "5.0", a numpy bool those of "True"
+    for a, b in ((["5"], [5]), (np.array(["5"]), np.array([5], dtype=np.uint32)), (np.array([5.0]), ["5.0"]),
+                 (np.array([True]), ["True"])):
+        ha, hb = pkg.IndexRationalBloomFilter(5000, 2.6), pkg.IndexRationalBloomFilter(5000, 2.6)
+        ha.add_indices(a)
+        hb.add_indices(b)
+        assert np.array_equal(ha.bit_array, hb.bit_array) and ha.bit_array.any(), (a, b)
 
 
 def test_inter_payloads_match_oracle_bytes_and_thread_count(pkg, co, tmp_path):
