@@ -194,11 +194,13 @@ class VideoFrameCompressor:
 
     def _estimate_noise_level(self, frame: np.ndarray) -> float:                  # ivc:727-746
         """N3: the 5x5 median runs on the device (k_median5, bit-exact with cv2.medianBlur); the float32 std is numpy's,
-        exactly as in the reference."""
+        exactly as in the reference.  An (h, w, 1) plane is filtered as (h, w), which is the shape cv2 returns for it; the
+        difference then broadcasts (h, w, 1) against (h, w) as the reference's does, so it raises ValueError unless numpy can
+        broadcast the two shapes."""
         a = np.ascontiguousarray(_frame_data(frame))
-        if a.ndim != 2 or a.dtype not in (np.uint8, np.uint16):
+        if not (a.ndim == 2 or (a.ndim == 3 and a.shape[2] == 1)) or a.dtype not in (np.uint8, np.uint16):
             raise NotImplementedError("noise estimate is implemented for 2-D uint8/uint16 planes (the Y / gray plane)")
-        smoothed = np.empty_like(a)
+        smoothed = np.empty(a.shape[:2], dtype=a.dtype)
         _cabi.check(_cabi.lib().rbf_median_blur5(_cabi.ctx(), _cabi.ptr(a), a.shape[0], a.shape[1], a.dtype.itemsize,
                                                  _cabi.ptr(smoothed)), _cabi.ctx())
         noise = a.astype(np.float32) - smoothed.astype(np.float32)                 # ivc:741
@@ -227,8 +229,9 @@ class VideoFrameCompressor:
         return ((x[:, :, 0] * 3735 + x[:, :, 1] * 19235 + x[:, :, 2] * 9798 + 16384) >> 15).astype(a.dtype)
 
     def _calculate_frame_diff(self, prev_frame, curr_frame, threshold: Optional[float] = None):
-        """ivc:768-847 -> (binary_diff uint8 HxW, changed_values, diff_density).  The mask is computed by K1: on the first
-        channel (Y) for `use_direct_yuv` frames, on the BGR->gray conversion otherwise (ivc:788-795), or on the single plane."""
+        """ivc:768-847 -> (binary_diff uint8, changed_values, diff_density).  The mask is computed by K1: on the first
+        channel (Y) for `use_direct_yuv` frames, on the BGR->gray conversion otherwise (ivc:788-795), or on the single plane.
+        It is H x W for colour frames and has the frame's shape otherwise, (h, w, 1) included (ivc:797-808)."""
         pd, cd = _frame_data(prev_frame), _frame_data(curr_frame)
         is_color = pd.ndim > 2 and pd.shape[2] > 1
         gray = is_color and not (self.use_direct_yuv and pd.shape[2] >= 3)
@@ -243,7 +246,7 @@ class VideoFrameCompressor:
         st.upload(np.stack([pd, cd]))
         res = st.encode([0], [1], float(threshold))[0]
         _, _, flat = st.fetch(0)                               # k1_only stream: the mask is the only output
-        binary_diff = flat.reshape(pd.shape[0], pd.shape[1]).astype(np.uint8)
+        binary_diff = flat.reshape(pd.shape[:2] if is_color else pd.shape).astype(np.uint8)
         vals = st.gather_changed(1)[0]                        # N1: ordered gather on the device (ivc:810-842)
         if is_color and self.use_direct_yuv and hasattr(curr_frame, "yuv_info"):
             changed = vals.astype(np.uint8)                   # ivc:825 allocates uint8: 16-bit samples are truncated there too
@@ -254,20 +257,34 @@ class VideoFrameCompressor:
         return binary_diff, changed, density
 
     def _apply_frame_diff(self, base_frame, diff_mask: np.ndarray, changed_values: np.ndarray):   # ivc:849-909
-        """N2: the scatter runs on the device (k_gather_scatter); the result is a copy of base_frame's type."""
+        """N2: the scatter runs on the device (k_gather_scatter); the result is a copy of base_frame's type.  Only mask entries
+        equal to 1 are applied (ivc:869).  Colour frames keep the base when the value count is not pixels x channels (ivc:882);
+        grayscale frames, (h, w, 1) included, follow numpy's `frame[mask == 1] = values` (ivc:906-907): one value is broadcast,
+        another count raises ValueError, and a mask without a set pixel leaves the frame as it is whatever the values.
+        Formats the device store does not hold, and values of another dtype, are applied by the same numpy indexing on the host."""
         nxt = base_frame.copy()
         data = _frame_data(nxt)
         vals = np.asarray(changed_values)
-        if data.dtype not in (np.uint8, np.uint16) or vals.dtype != data.dtype or not (data.ndim == 2 or data.shape[2] == 3):
-            rows, cols = np.where(diff_mask == 1)              # formats outside the device store: host indexing
-            ch = data.shape[2] if data.ndim == 3 else 1
-            if len(vals) == len(rows) * ch:
-                data[rows, cols] = vals.reshape(-1, ch) if ch > 1 else vals
-        else:
+        sel = np.asarray(diff_mask) == 1                       # ivc:869
+        color = data.ndim == 3 and data.shape[2] > 1
+        device = (data.dtype in (np.uint8, np.uint16) and vals.dtype == data.dtype and vals.ndim == 1 and
+                  data.ndim in (2, 3) and (data.ndim == 2 or data.shape[2] in (1, 3)) and
+                  sel.shape == (data.shape[:2] if color else data.shape))
+        if device and not color and vals.size != np.count_nonzero(sel):
+            device = False                                     # numpy decides: a broadcast, a ValueError or an empty mask
+        if device:
             st = self._stream_for(data.shape, data.dtype, k1_only=True)
             st.upload(np.ascontiguousarray(data)[None], first=0)
-            st.apply_diff(0, 1, diff_mask, vals)               # value-count mismatch leaves the base unchanged (ivc:882)
-            data[...] = st.download(1)
+            st.apply_diff(0, 1, sel, vals)                     # value-count mismatch leaves the base unchanged (ivc:882)
+            data[...] = st.download(1).reshape(data.shape)
+        elif color:                                            # ivc:872-903
+            rows, cols = np.nonzero(sel)
+            if len(vals) == len(rows) * data.shape[2]:
+                data[rows, cols] = vals.reshape(-1, data.shape[2])
+        else:                                                  # ivc:904-907
+            idx = np.nonzero(sel)
+            if len(idx[0]) > 0:
+                data[idx] = vals
         if self.use_direct_yuv and hasattr(nxt, "yuv_info") and data.ndim == 3:
             nxt.yuv_info["y_plane"] = data[:, :, 0].copy()
             nxt.yuv_info["u_plane"] = data[:, :, 1].copy()

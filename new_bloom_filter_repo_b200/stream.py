@@ -176,9 +176,18 @@ class FrameStream:
         return out
 
     def apply_diff(self, base_frame: int, out_frame: int, mask: np.ndarray, values: np.ndarray) -> int:
-        """store[out_frame] = store[base_frame] with masked pixels replaced by `values` (ivc:849-909); returns pixels applied."""
-        mk = np.packbits(np.ascontiguousarray(mask, dtype=np.uint8).reshape(-1), bitorder="little")
-        vals = np.ascontiguousarray(values).view(np.uint8).reshape(-1)
+        """store[out_frame] = store[base_frame] with the pixels where `mask` is non-zero replaced by `values`, C samples of the
+        stream's dtype per pixel in row-major order; returns pixels applied.  When values does not hold exactly C samples per set
+        pixel, out_frame is a copy of base_frame and 0 is returned (ivc:882).  VideoFrameCompressor._apply_frame_diff passes
+        `mask == 1` (ivc:869)."""
+        m = np.asarray(mask)
+        if m.size != self.npix:
+            raise ValueError(f"a mask of {m.size} entries for frames of {self.npix} pixels")
+        v = np.asarray(values)
+        if v.dtype != self.dtype:
+            raise ValueError(f"values of dtype {v.dtype} for a stream of {self.dtype}")
+        mk = np.packbits((m != 0).reshape(-1), bitorder="little")
+        vals = np.ascontiguousarray(v).view(np.uint8).reshape(-1)
         applied = C.c_uint64()
         _cabi.check(_cabi.lib().rbf_stream_apply_diff(self._h, int(base_frame), int(out_frame), _cabi.ptr(mk),
                                                       _cabi.ptr(vals) if vals.size else None, vals.size, C.byref(applied)), _cabi.ctx())

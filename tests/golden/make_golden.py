@@ -403,9 +403,129 @@ def gen_gray():
                            "cube_u16_sha256": sha(cv2.cvtColor(cube16, cv2.COLOR_BGR2GRAY)), "cv2_version": cv2.__version__})
 
 
+def enc(a: np.ndarray) -> dict:
+    """An array as {"shape", "dtype", "hex"} (read back by tests/test_gpu_frame_api.py)."""
+    a = np.ascontiguousarray(a)
+    return {"shape": list(a.shape), "dtype": a.dtype.name, "hex": a.tobytes().hex()}
+
+
+def outcome(fn):
+    """-> ("ok", result) or ("error", the exception's type name)."""
+    try:
+        return "ok", fn()
+    except Exception as e:                                # the reference's own exception is the recorded outcome
+        return "error", type(e).__name__
+
+
+def gen_frame_api():
+    """VideoFrameCompressor's per-frame API (ivc:727-909) at its mask value, value count, layout and adaptive-threshold edges:
+    inputs, and the SHA-256 of every result or the name of the exception the reference raises."""
+    import cv2
+    rng = np.random.default_rng(2026)
+    h, w = 6, 7
+    apply_cases, diff_cases, noise_cases = [], [], []
+
+    def base_for(shape, dt):
+        return rng.integers(0, 256 if dt == np.uint8 else 65536, shape).astype(dt)
+
+    # mask values: only entries == 1 are applied (ivc:869)
+    masks = {}
+    m = np.zeros((h, w), np.uint8); m[1, 1] = 1; m[3, 4] = 1; m[5, 6] = 1; masks["bin"] = m
+    m = np.zeros((h, w), np.uint8); m[1, 1] = 1; m[2, 2] = 255; masks["u8_255"] = m
+    m = np.zeros((h, w), np.uint8); m[1, 1] = 1; m[4, 0] = 2; m[0, 6] = 1; masks["u8_2"] = m
+    m = np.zeros((h, w), np.int16); m[1, 1] = 1; m[2, 2] = 257; m[3, 3] = -1; masks["i16"] = m
+    m = np.zeros((h, w), np.float64); m[1, 1] = 1.0; m[2, 2] = 0.5; m[5, 0] = 1.0; masks["f64"] = m
+    m = np.zeros((h, w), bool); m[0, 0] = True; m[2, 3] = True; masks["bool"] = m
+    masks["empty"] = np.zeros((h, w), np.uint8)
+
+    def counts(n):                                        # value counts in pixels: exact, short, long, none, one
+        return {"exact": n, "short": n - 1, "long": n + 1, "zero": 0, "one": 1}
+
+    layouts = [("g8", (h, w), np.uint8, False), ("g16", (h, w), np.uint16, False), ("g1", (h, w, 1), np.uint8, False),
+               ("c8", (h, w, 3), np.uint8, False), ("c16", (h, w, 3), np.uint16, False), ("c4", (h, w, 4), np.uint8, False),
+               ("yuv8", (h, w, 3), np.uint8, True), ("yuv16", (h, w, 3), np.uint16, True)]
+    picks = [("g8", "bin", ["exact", "short", "long", "zero", "one"]), ("g8", "u8_255", ["exact", "long"]),
+             ("g8", "empty", ["long", "zero"]), ("g16", "i16", ["exact", "one"]), ("g16", "f64", ["exact", "long"]),
+             ("g1", "bin", ["exact", "short", "one"]), ("g1", "u8_2", ["exact"]), ("c8", "bin", ["exact", "short", "one"]),
+             ("c8", "u8_255", ["exact", "long"]), ("c16", "i16", ["exact"]), ("c16", "bool", ["exact", "zero"]),
+             ("c4", "u8_2", ["exact", "short"]), ("yuv8", "bin", ["exact", "short"]), ("yuv8", "f64", ["exact"]),
+             ("yuv16", "bin", ["exact"]), ("yuv16", "u8_255", ["long"])]
+    lay = {name: (shape, dt, yuv) for name, shape, dt, yuv in layouts}
+    for lname, mname, cnames in picks:
+        shape, dt, yuv = lay[lname]
+        base = base_for(shape, dt)
+        mask = masks[mname]
+        if len(shape) == 3 and shape[2] == 1:
+            mask = mask[:, :, None]                       # the (h, w, 1) mask _calculate_frame_diff returns for such frames
+        ch = shape[2] if len(shape) == 3 and shape[2] > 1 else 1
+        n = int(np.sum(mask == 1))
+        for cname in cnames:
+            k = counts(n)[cname]
+            vdt = np.uint8 if yuv else dt                 # YUV values are u8 (ivc:825)
+            vals = rng.integers(0, 256 if vdt == np.uint8 else 65536, max(0, k) * ch).astype(vdt)
+            vfc = refshim.make_vfc(ivc, use_direct_yuv=yuv)
+            frame = vfc_wrap(base.copy()) if yuv else base.copy()
+            status, res = outcome(lambda: vfc._apply_frame_diff(frame, mask, vals))
+            rec = {"name": f"{lname}/{mname}/{cname}", "use_direct_yuv": yuv, "yuv": yuv, "base": enc(base), "mask": enc(mask),
+                   "values": enc(vals)}
+            if status == "error":
+                rec["error"] = res
+            else:
+                d = np.asarray(res.data if hasattr(res, "yuv_info") else res)
+                rec.update(result_shape=list(d.shape), result_dtype=d.dtype.name, result_sha256=sha(d))
+                if yuv:
+                    rec["planes_sha256"] = [sha(res.yuv_info[p]) for p in ("y_plane", "u_plane", "v_plane")]
+                rec["base_unchanged"] = bool(np.array_equal(np.asarray(frame.data if yuv else frame), base))
+            apply_cases.append(rec)
+
+    # _calculate_frame_diff across its branches (ivc:768-847)
+    def pair(shape, dt, p=0.3):
+        prev = base_for(shape, dt)
+        curr = prev.copy()
+        sel = rng.random(shape[:2]) < p
+        hi = 256 if dt == np.uint8 else 65536
+        curr[sel] = (curr[sel].astype(np.int64) + rng.integers(1, 8, curr[sel].shape)) % hi
+        return prev, curr
+
+    for name, shape, dt, yuv, thr in [("yuv8_thr3", (9, 11, 3), np.uint8, True, 3.0), ("yuv16_thr3.5", (9, 11, 3), np.uint16, True, 3.5),
+                                      ("arr3_direct_thr0", (9, 11, 3), np.uint8, "array", 0.0), ("bgr8_thr3", (9, 11, 3), np.uint8, False, 3.0),
+                                      ("bgr16_thr3.5", (9, 11, 3), np.uint16, False, 3.5), ("g8_thr0", (9, 11), np.uint8, False, 0.0),
+                                      ("g16_none", (12, 17), np.uint16, False, None), ("g1_thr3", (9, 11, 1), np.uint8, False, 3.0),
+                                      ("g1_none", (9, 11, 1), np.uint8, False, None), ("g1_square_none", (6, 6, 1), np.uint8, False, None),
+                                      ("yuv8_none", (12, 17, 3), np.uint8, True, None), ("bgr8_none", (12, 17, 3), np.uint8, False, None)]:
+        prev, curr = pair(shape, dt)
+        vfc = refshim.make_vfc(ivc, use_direct_yuv=bool(yuv))
+        pf, cf = (vfc_wrap(prev), vfc_wrap(curr)) if yuv is True else (prev, curr)
+        status, res = outcome(lambda: vfc._calculate_frame_diff(pf, cf, threshold=thr))
+        rec = {"name": name, "use_direct_yuv": bool(yuv), "yuv": yuv is True, "threshold": thr, "prev": enc(prev), "curr": enc(curr)}
+        if status == "error":
+            rec["error"] = res
+        else:
+            mask, changed, dens = res
+            rec.update(mask_shape=list(mask.shape), mask_sha256=sha(mask.astype(np.uint8)), changed_dtype=changed.dtype.name,
+                       changed_sha256=sha(changed), changed_len=int(len(changed)), density=float(dens).hex())
+        diff_cases.append(rec)
+
+    # noise level and adaptive threshold where cv2.medianBlur is the reference's median (ivc:727-766)
+    for name, plane, tol in [("u8_random", base_for((9, 11), np.uint8), 10.0), ("u16_high", (base_for((8, 13), np.uint16) | 0x8000), 0.001),
+                             ("u8_ties", rng.choice(np.array([0, 128, 255], np.uint8), (16, 33)), 0.05),
+                             ("u16_ties", rng.choice(np.array([0, 32767, 32768, 65535], np.uint16), (17, 31)), 0.0001),
+                             ("u8_flat", np.full((7, 9), 200, np.uint8), 10.0), ("u8_1x1", np.array([[77]], np.uint8), 10.0)]:
+        vfc = refshim.make_vfc(ivc, noise_tolerance=tol)
+        nl = vfc._estimate_noise_level(plane)
+        thr = vfc._adaptive_diff_threshold(plane)
+        noise_cases.append({"name": name, "plane": enc(plane), "noise_tolerance": tol, "noise_level": float(nl).hex(),
+                            "noise_level_type": type(nl).__name__, "threshold": float(thr).hex(),
+                            "median_sha256": sha(cv2.medianBlur(plane, 5))})
+    dump("frame_api_kat.json", {"apply": apply_cases, "diff": diff_cases, "noise": noise_cases, "cv2_version": cv2.__version__})
+
+
 if __name__ == "__main__":
     if "--gray-only" in sys.argv:
         gen_gray()
+        sys.exit(0)
+    if "--frame-api-only" in sys.argv:
+        gen_frame_api()
         sys.exit(0)
     gen_gray()
     gen_xxh64()
@@ -417,3 +537,4 @@ if __name__ == "__main__":
     gen_strings()
     gen_keyframes()
     gen_adaptive()
+    gen_frame_api()
