@@ -428,12 +428,18 @@ __global__ void __launch_bounds__(Q2_THREADS, 1) k_query2(const FrameJob* __rest
 //   * TY = 5 (half-decade tiles): records {idx:24, lane:5, y:3} -- filters up to 2^24 bits (8K frames at k* = 4) stay on the
 //     tile kernel; with the carry, half tiles no longer pay for half-full batches.
 //   * one digit-constant table per CTA instead of one per warp.
+//   * full-decade tiles run stage B two full batches at a time (two independent hash-and-probe chains per lane), so a warp
+//     waits for the probes of both batches at once (with floor_k = 3, four loads in flight instead of two).
 // Results are identical to every other formulation (the variant matrix in tests/test_gpu_parity.py).
 // ------------------------------------------------------------------------------------------
 #ifndef RBF_Q4_WARPS
 #define RBF_Q4_WARPS 28
 #endif
 constexpr int Q4_WARPS = RBF_Q4_WARPS, Q4_THREADS = 32 * Q4_WARPS;
+// Full-decade tiles launch 24 of them by default: stage B keeps two batches in flight, so fewer warps still cover its latency,
+// and the scratch of the four warps left out (9.7 KB) holds more of the bit array on chip, which takes probes off the L2 tail.
+// Measured faster than 20, 22 and 28 warps at 4K.  Half-decade tiles run stage B one batch deep and keep all Q4_WARPS.
+constexpr int Q4_FULL_TILE_WARPS = 24;
 constexpr int Q4_TABLE_WORDS = 32;                                     // 10 x uint64 digit constants, padded
 template <int TY> struct Q4Cfg {
     static constexpr int BUF = 32 * TY + 32;                            // a tile's survivors (worst case) + carried records (< 32)
@@ -506,6 +512,36 @@ __device__ __noinline__ void query_slab_tiled2(const FilterK K, uint32_t sm_addr
             uint32_t nproc = last_tile ? tot2 : (tot2 & ~31u);
             if (nproc == 0u && rem != 0u) nproc = tot2;              // a record is carried over one tile at most
             const uint32_t yoff = (uint32_t)(h * TY);
+            // the owner's decade state of seed 2 for a record; the batch at b == 0 holds the carried records (g < rem), which
+            // fetch the state, x and y offset of the tile they came from
+            auto owner_state = [&](const uint32_t b, const uint32_t g, const uint32_t owner, uint32_t& y, uint32_t& xr) {
+                uint64_t D2o = (uint64_t)__shfl_sync(0xffffffffu, (uint32_t)D2, owner) |
+                               ((uint64_t)__shfl_sync(0xffffffffu, (uint32_t)(D2 >> 32), owner) << 32);
+                if (b == 0u && rem != 0u) {                          // warp-uniform
+                    const uint64_t D2q = (uint64_t)__shfl_sync(0xffffffffu, (uint32_t)D2p, owner) |
+                                         ((uint64_t)__shfl_sync(0xffffffffu, (uint32_t)(D2p >> 32), owner) << 32);
+                    if (g < rem) { D2o = D2q; y += yoffp - yoff; xr = xp; }
+                }
+                return D2o;
+            };
+            auto h2_step = [&](const uint64_t D2o, const uint32_t y) {
+                uint64_t rb = 0;
+                if (kind_ends_in_byte<KIND>()) { const uint2 t = lds64(rb_addr + 8u * y); rb = (uint64_t)t.x | ((uint64_t)t.y << 32); }
+                return mod_fast(finish_prep<KIND>(D2o, K.s2, y, rb), K.fm, K.nm);
+            };
+            // a batch's survivors of probes 1..floor_k-1: through the C ring (drained as soon as it holds 32, so it never holds
+            // more than 63) or straight into the pass bits
+            auto push_c = [&](uint32_t idx, const uint32_t stepm, const uint32_t ok, const uint32_t tag) {
+                if (K.has_act) {
+                    idx = addmod_fast(idx, stepm, K.fm.m);           // index of probe floor_k
+                    const uint32_t b2 = __ballot_sync(0xffffffffu, ok != 0u);
+                    sts64_if(qc_addr + 8u * ((qc_head + qc_cnt + __popc(b2 & lt)) & (Q2_RING - 1)), idx, tag, ok != 0u);
+                    qc_cnt += __popc(b2);
+                    if (qc_cnt >= 32u) drain_c_ring<KIND, PM>(K, sm_addr, 0u, gl, sm_words, qc_addr, pacc_addr, lane, CA, qc_head, qc_cnt);
+                } else {
+                    deliver_pass(pacc_addr, tag, ok != 0u);
+                }
+            };
             // one batch of 32 records; FULL batches (all but the last of a slab) carry no per-lane validity logic
             auto stage_b = [&](const uint32_t b, auto full) {
                 constexpr bool FULL = decltype(full)::value;
@@ -514,17 +550,9 @@ __device__ __noinline__ void query_slab_tiled2(const FilterK K, uint32_t sm_addr
                 const uint32_t rec = lds32(buf_addr + 4u * (FULL ? g : min(g, (uint32_t)(Cfg::BUF - 1))));
                 const uint32_t owner = (rec >> Cfg::IDXB) & 31u;
                 uint32_t y = (rec >> (Cfg::IDXB + 5)) + yoff, xr = x;
-                uint64_t D2o = (uint64_t)__shfl_sync(0xffffffffu, (uint32_t)D2, owner) |
-                               ((uint64_t)__shfl_sync(0xffffffffu, (uint32_t)(D2 >> 32), owner) << 32);
-                if (b == 0u && rem != 0u) {                          // warp-uniform: the batch that holds the carried records
-                    const uint64_t D2q = (uint64_t)__shfl_sync(0xffffffffu, (uint32_t)D2p, owner) |
-                                         ((uint64_t)__shfl_sync(0xffffffffu, (uint32_t)(D2p >> 32), owner) << 32);
-                    if (g < rem) { D2o = D2q; y = (rec >> (Cfg::IDXB + 5)) + yoffp; xr = xp; }
-                }
+                const uint64_t D2o = owner_state(b, g, owner, y, xr);
                 if (!have) y = 0u;
-                uint64_t rb = 0;
-                if (kind_ends_in_byte<KIND>()) { const uint2 t = lds64(rb_addr + 8u * y); rb = (uint64_t)t.x | ((uint64_t)t.y << 32); }
-                const uint32_t stepm = have ? mod_fast(finish_prep<KIND>(D2o, K.s2, y, rb), K.fm, K.nm) : 0u;
+                const uint32_t stepm = have ? h2_step(D2o, y) : 0u;
                 uint32_t idx = have ? (rec & IDXM) : 0u;
                 uint32_t ok = have ? 1u : 0u;
                 if (FKT > 0) {
@@ -539,18 +567,36 @@ __device__ __noinline__ void query_slab_tiled2(const FilterK K, uint32_t sm_addr
                         ok &= probe_bit<PM>(sm_addr, 0u, gl, sm_words, idx);
                     }
                 }
-                const uint32_t tag = (owner << 8) | (xr << 4) | y;
-                if (K.has_act) {
-                    idx = addmod_fast(idx, stepm, K.fm.m);           // index of probe floor_k
-                    const uint32_t b2 = __ballot_sync(0xffffffffu, ok != 0u);
-                    sts64_if(qc_addr + 8u * ((qc_head + qc_cnt + __popc(b2 & lt)) & (Q2_RING - 1)), idx, tag, ok != 0u);
-                    qc_cnt += __popc(b2);
-                    if (qc_cnt >= 32u) drain_c_ring<KIND, PM>(K, sm_addr, 0u, gl, sm_words, qc_addr, pacc_addr, lane, CA, qc_head, qc_cnt);
-                } else {
-                    deliver_pass(pacc_addr, tag, ok != 0u);
+                push_c(idx, stepm, ok, (owner << 8) | (xr << 4) | y);
+            };
+            // two full batches (records b + lane and b + 32 + lane) as two independent chains, so that a warp waits for the
+            // probes of both at once: with part of the array in L2 nearly every batch holds an L2 probe.  Only the first
+            // batch can hold carried records (b == 0, g < rem < 32).
+            auto stage_b2 = [&](const uint32_t b) {
+                const uint32_t rec0 = lds32(buf_addr + 4u * (b + lane)), rec1 = lds32(buf_addr + 4u * (b + 32u + lane));
+                const uint32_t own0 = (rec0 >> Cfg::IDXB) & 31u, own1 = (rec1 >> Cfg::IDXB) & 31u;
+                uint32_t y0 = (rec0 >> (Cfg::IDXB + 5)) + yoff, x0 = x;
+                const uint32_t y1 = (rec1 >> (Cfg::IDXB + 5)) + yoff;
+                const uint64_t D2o0 = owner_state(b, b + lane, own0, y0, x0);
+                const uint64_t D2o1 = (uint64_t)__shfl_sync(0xffffffffu, (uint32_t)D2, own1) |
+                                      ((uint64_t)__shfl_sync(0xffffffffu, (uint32_t)(D2 >> 32), own1) << 32);
+                const uint32_t st0 = h2_step(D2o0, y0), st1 = h2_step(D2o1, y1);
+                uint32_t idx0 = rec0 & IDXM, idx1 = rec1 & IDXM, ok0 = 1u, ok1 = 1u;
+#pragma unroll
+                for (int i = 1; i < FKT; i++) {
+                    idx0 = addmod_fast(idx0, st0, K.fm.m);
+                    idx1 = addmod_fast(idx1, st1, K.fm.m);
+                    ok0 &= probe_bit<PM>(sm_addr, 0u, gl, sm_words, idx0);
+                    ok1 &= probe_bit<PM>(sm_addr, 0u, gl, sm_words, idx1);
                 }
+                push_c(idx0, st0, ok0, (own0 << 8) | (x0 << 4) | y0);
+                push_c(idx1, st1, ok1, (own1 << 8) | (x << 4) | y1);
             };
             uint32_t bb = 0;
+            if (FKT > 0 && TY == 10) {                               // half tiles: a second chain spills at 72 registers
+#pragma unroll 1
+                for (; bb + 64u <= nproc; bb += 64u) stage_b2(bb);
+            }
 #pragma unroll 1
             for (; bb + 32u <= nproc; bb += 32u) stage_b(bb, std::true_type{});
             if (bb < nproc) stage_b(bb, std::false_type{});
@@ -590,7 +636,7 @@ __global__ void __launch_bounds__(Q4_THREADS, 1) k_query4(const FrameJob* __rest
     const uint32_t rb_addr = smem_u32(dyn);                                    // digit constants, one table per CTA
     const uint32_t buf = smem_u32(dyn + Q4_TABLE_WORDS + warp * Cfg::WARP_WORDS);
     const uint32_t pacc = buf + 4u * Cfg::BUF + 8u * Q2_RING;
-    const uint32_t nwarps = blockDim.x >> 5;                                   // <= Q4_WARPS (register budget); fewer when K2 runs beside
+    const uint32_t nwarps = blockDim.x >> 5;                                   // <= Q4_WARPS (register budget); Q4_FULL_TILE_WARPS by default for full tiles
     uint32_t* sbits = dyn + Q4_TABLE_WORDS + nwarps * Cfg::WARP_WORDS;
     const uint32_t sb_addr = smem_u32(sbits);
     sts128_if(pacc + 16u * lane, 0u, 0u, 0u, 0u, true);

@@ -283,13 +283,14 @@ cudaError_t launch_query(LaunchCfg& L, const FrameJob* d_jobs, const uint32_t* d
                          uint32_t max_l_bits, cudaStream_t st) {
     if (F <= 0 || total_centuries == 0) return cudaSuccess;
     int variant = L.query_variant, tile_warps = L.query_warps;
-    if (tile_warps < 4 || tile_warps > Q4_WARPS) tile_warps = Q4_WARPS;
+    if (tile_warps < 4 || tile_warps > Q4_WARPS) tile_warps = 0;                       // 0: the tile width's default
     int cap = L.query_smem_cap & ~15;
     if (cap > query_max_smem_bytes()) cap = query_max_smem_bytes() & ~15;
     const uint32_t need_words = (((max_l_bits + 31u) >> 5) + 3u) & ~3u;
     if (variant >= 2 && variant <= 4) variant = 5;
     if (variant >= 5 && max_l_bits <= (1u << 24)) {       // decade tiles (full stage-B batches with carry)
         const bool half = (variant == 6) || max_l_bits > (1u << 23);      // half-decade tiles: 24-bit record indices
+        if (tile_warps == 0) tile_warps = half ? Q4_WARPS : Q4_FULL_TILE_WARPS;
         const int qbytes = 4 * (Q4_TABLE_WORDS + tile_warps * (half ? Q4Cfg<5>::WARP_WORDS : Q4Cfg<10>::WARP_WORDS));
         if (cap < qbytes + 1024) cap = qbytes + 1024;
         const int bits_cap = cap - qbytes;

@@ -107,7 +107,7 @@ struct LaunchCfg {
     int query_variant = 5;         // 0: per-lane; 1: staged A->B->C rings, L2 tail; 2, 3, 4: as 5; 5: decade tiles with carried stage-B
                                    // batches (half tiles for 2^23 < m <= 2^24, ring kernel beyond); 6: half-decade tiles for every m <= 2^24
     int query_smem_cap = 0;
-    int query_warps = 0;           // warps per CTA of the tile query kernel (0 = its compiled maximum, 28)
+    int query_warps = 0;           // warps per CTA of the tile query kernel (0 = default: 24 for full-decade tiles, 28 for half ones)
     int k2_clusters[9] = {0};      // resident K2 clusters of 1..8 CTAs, measured by the first K2 launch of each shape.  Not at
                                    // creation: querying it there slowed 8K K3 (which never uses this kernel) by 12 %, cause unknown
     int64_t launches = 0;          // kernels enqueued (rbf_get_counter "kernel_launches")
