@@ -272,6 +272,32 @@ int rbf_zlib_compress_batch(rbf_ctx* ctx, uint32_t count, const void* const* src
  * the device, one zlib stream per pair (the raw values never cross PCIe); out_offsets[pairs+1] as above */
 int rbf_stream_zlib_changed(rbf_stream* s, uint32_t pairs, uint8_t* out_host, uint64_t out_capacity, uint64_t* out_offsets);
 
+/* ---- inflate of streams in the layout above.  Each 64 KiB segment starts at offset 2 or right after a 00 00 FF FF, so every
+ *     such offset is inflated on the device as a candidate and the host follows the chain of accepted segments to the trailer.
+ *     A stream the device declines is a normal outcome (on_device[i] = 0): not 78 9C, a segment outside the layout (fixed-Huffman
+ *     blocks, BFINAL 1, matches before the segment start, ...), a segment other than the last not inflating to 65536 bytes,
+ *     anything but 03 00 and the right Adler-32 after the last segment, bytes after the trailer, more candidate starts than
+ *     2 ceil(bounds[i] / 65536) + 8, or more than bounds[i] inflated bytes.  The caller inflates declined streams another way.
+ * rbf_inflate_segment: the segment inflater the kernels run, on the host (no context, no GPU): one segment at in[0] with avail
+ * bytes of the stream left, into out[65536].  *status 0 = accepted (dynamic or stored blocks with BFINAL 0 up to the first empty
+ * stored block); anything else is refused with a non-zero status, never reading in[avail..) or writing out[65536..).  consumed:
+ * bytes through the closing 00 00 FF FF; produced: output bytes; s1, s2: their Adler-32 sums from (0, 0). */
+int rbf_inflate_segment(const uint8_t* in, uint64_t avail, uint8_t* out, uint32_t* status, uint64_t* consumed, uint32_t* produced,
+                        uint32_t* s1, uint32_t* s2);
+/* host streams srcs[count] of lens[count] bytes (one H2D copy of each) -> the inflated bytes of the accepted ones back to back
+ * in out_host: stream i is out_host[out_offsets[i], out_offsets[i+1]), empty when on_device[i] == 0.  A stream whose output
+ * does not fit the capacity left after the earlier ones is declined too; out_capacity >= the sum of bounds[i] fits them all. */
+int rbf_zlib_decompress_batch(rbf_ctx* ctx, uint32_t count, const void* const* srcs, const uint64_t* lens, const uint64_t* bounds,
+                              uint8_t* out_host, uint64_t out_capacity, uint64_t* out_offsets /* count+1 */, uint8_t* on_device);
+/* the value streams of a decoded group (bounds[i]: pair i's value bytes, vcount x sample bytes): inflated into a device buffer of
+ * the stream, the accepted ones back to back, out_lens[i] bytes each (0 when declined).  rbf_stream_apply_chain_inflated then
+ * runs rbf_stream_apply_chain_motion on them (value_offsets[count] must not exceed what was placed; fields may be NULL when no
+ * mode is 2), so the inflated values never cross PCIe.  The next inflate_values, or the apply, ends their use. */
+int rbf_stream_inflate_values(rbf_stream* s, uint32_t count, const void* const* srcs, const uint64_t* lens, const uint64_t* bounds,
+                              uint64_t* out_lens, uint8_t* on_device);
+int rbf_stream_apply_chain_inflated(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint64_t* value_offsets,
+                                    const uint8_t* modes, const int8_t* fields, uint64_t* applied_out);
+
 /* ------------------------------------------------------------------ multi-GPU (one process per GPU)
  * frames are sharded across ranks; the per-rank Bloom bit arrays are exchanged with ONE ncclAllGather
  * over NVLink.  NCCL is dlopen'ed (libnccl.so.2); the unique id travels over the caller's own channel. */

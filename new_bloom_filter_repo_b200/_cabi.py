@@ -52,6 +52,7 @@ EXPORTS = [
     "rbf_stream_decode_masks", "rbf_stream_apply_chain", "rbf_stream_apply_chain_modes", "rbf_stream_apply_chain_motion",
     "rbf_stream_motion_search", "rbf_stream_download_batch",
     "rbf_zlib_bound", "rbf_deflate_code_lengths", "rbf_zlib_compress_batch", "rbf_stream_zlib_changed",
+    "rbf_inflate_segment", "rbf_zlib_decompress_batch", "rbf_stream_inflate_values", "rbf_stream_apply_chain_inflated",
     "rbf_nccl_unique_id", "rbf_nccl_init", "rbf_nccl_allgather", "rbf_stream_allgather_bitmaps", "rbf_nccl_destroy",
     "rbf_peer_export", "rbf_peer_open", "rbf_peer_close", "rbf_peer_gather_init", "rbf_peer_gather_half", "rbf_peer_gather_shutdown",
 ]
@@ -133,6 +134,10 @@ def _sig(L):
     L.rbf_deflate_code_lengths.argtypes = [vp, u32, u32, vp]
     L.rbf_zlib_compress_batch.argtypes = [vp, u32, vp, vp, i32, vp, u64, vp]
     L.rbf_stream_zlib_changed.argtypes = [vp, u32, vp, u64, vp]
+    L.rbf_inflate_segment.argtypes = [vp, u64, vp, P(u32), P(u64), P(u32), P(u32), P(u32)]
+    L.rbf_zlib_decompress_batch.argtypes = [vp, u32, vp, vp, vp, vp, u64, vp, vp]
+    L.rbf_stream_inflate_values.argtypes = [vp, u32, vp, vp, vp, vp, vp]
+    L.rbf_stream_apply_chain_inflated.argtypes = [vp, u32, u32, vp, vp, vp, vp]
     L.rbf_nccl_unique_id.argtypes = [vp]
     L.rbf_nccl_init.argtypes = [vp, vp, i32, i32]
     L.rbf_nccl_allgather.argtypes = [vp, vp, vp, u64]
@@ -221,6 +226,17 @@ def optimal_params(n: int, ones: int):
 def zlib_bound(n: int) -> int:
     """Worst-case size of the zlib stream the device coder writes for n input bytes."""
     return int(lib().rbf_zlib_bound(int(n)))
+
+
+def inflate_segment(data, offset: int = 0):
+    """The device inflater of one segment (host build): data[offset:] is the rest of the stream.
+    -> (status, consumed, output bytes, s1, s2); status 0 = accepted."""
+    buf = np.frombuffer(memoryview(data).cast("B"), dtype=np.uint8)[offset:]
+    out = np.zeros(65536, dtype=np.uint8)
+    st, used, n, s1, s2 = C.c_uint32(), C.c_uint64(), C.c_uint32(), C.c_uint32(), C.c_uint32()
+    check(lib().rbf_inflate_segment(ptr(buf) if buf.size else None, buf.size, ptr(out), C.byref(st), C.byref(used), C.byref(n),
+                                    C.byref(s1), C.byref(s2)))
+    return int(st.value), int(used.value), out[:n.value].tobytes(), int(s1.value), int(s2.value)
 
 
 def deflate_code_lengths(freqs, max_bits: int) -> np.ndarray:

@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "librbf_b200.so")
 SOURCES = ["rbf_kernels.cu", "rbf_api.cu"]
 HEADERS = ["rbf_hash.cuh", "rbf_kernels.cuh", "rbf_k1_threshold.cuh", "rbf_k2_insert.cuh", "rbf_k3_query.cuh", "rbf_k3b_witness.cuh",
-           "rbf_aux_kernels.cuh", "rbf_deflate.cuh", "rbf_k4c_apply.cuh", "rbf_motion.cuh", os.path.join("..", "..", "include", "rbf_b200.h")]
+           "rbf_aux_kernels.cuh", "rbf_deflate.cuh", "rbf_inflate.cuh","rbf_k4c_apply.cuh", "rbf_motion.cuh", os.path.join("..", "..", "include", "rbf_b200.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -8,7 +8,9 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/rbf_b200.h"
@@ -88,6 +90,7 @@ enum ScratchSlot {
     kScrGatherCounts,                             // per-chunk set-bit counts of the gather / scatter kernels
     kScrZlibRes, kScrZlibOut, kScrZlibStage, kScrZlibSegs, kScrZlibCopies, kScrZlibSmall, kScrZlibIn,
     kScrDecodeCounts, kScrChainSmall, kScrChainTiles,   // decode_masks' counts; apply_chain's offsets + flags + totals, tile prefix
+    kScrInflateIn, kScrInflateSmall, kScrInflateSlots, kScrInflateRes, kScrInflateOut,   // inflate_streams / inflate_place
 };
 
 static int scratch_get(rbf_ctx* c, int slot, size_t bytes, void** out) {
@@ -613,6 +616,9 @@ struct rbf_stream {
     int motion_values = 0;  // 1: the gathers return residuals against the motion-compensated previous frame of the last search
     int8_t* d_fields = nullptr;             // [max_pairs][mv_blocks(H, W)][2] block vectors of rbf_stream_motion_search
     uint32_t motion_pairs = 0;              // pairs searched since the last encode (0: none, or a decode_masks overwrote the slots)
+    uint8_t* d_inflated = nullptr;          // rbf_stream_inflate_values: the group's values back to back, read by apply_chain_inflated
+    size_t inflated_cap = 0;
+    uint64_t inflated_bytes = 0;            // bytes the last rbf_stream_inflate_values placed (cleared by apply_chain_inflated)
     bool last_k1_only = false;
     rbf_seeds last_sd = {};                 // seeds of the last encode (decode_verify rebuilds its jobs from them and last_infos)
     size_t bits_hwm = 0, wit_hwm = 0;   // bytes per slot that may hold set bits (see enc_stage_jobs)
@@ -626,7 +632,7 @@ extern "C" void rbf_stream_destroy(rbf_stream* s) {
     cudaSetDevice(s->c->device);
     cudaFree(s->d_frames); cudaFree(s->d_mask); cudaFree(s->d_bits); cudaFree(s->d_wit); cudaFree(s->d_pass); cudaFree(s->d_dec);
     cudaFree(s->d_jobs); cudaFree(s->d_pairs); cudaFree(s->d_prefix); cudaFree(s->d_ones); cudaFree(s->d_resid); cudaFree(s->d_wlen); cudaFree(s->d_chunkcnt);
-    cudaFree(s->d_fields);
+    cudaFree(s->d_fields); cudaFree(s->d_inflated);
     for (auto& e : s->ev) if (e) cudaEventDestroy(e);
     for (auto& e : s->ev_copy) if (e) cudaEventDestroy(e);
     cudaFreeHost(s->h_jobs); cudaFreeHost(s->h_pairs); cudaFreeHost(s->h_prefix); cudaFreeHost(s->h_ones); cudaFreeHost(s->h_resid); cudaFreeHost(s->h_wlen);
@@ -1349,8 +1355,10 @@ extern "C" int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32
 }
 
 // rbf_stream_apply_chain_modes / _motion: modes[i] <= max_mode (NULL: every pair plain); fields [count][nblocks][2] for mode 2 pairs
+// d_values (device): the values are already there, as rbf_stream_inflate_values leaves them, and `values` is not read
 static int apply_chain_impl(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values, const uint64_t* value_offsets,
-                            const uint8_t* modes, uint8_t max_mode, const int8_t* fields, uint64_t* applied_out) {
+                            const uint8_t* modes, uint8_t max_mode, const int8_t* fields, uint64_t* applied_out,
+                            const uint8_t* d_values = nullptr) {
     if (!s || !value_offsets || !applied_out) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_apply_chain: NULL");
     rbf_ctx* c = s->c;
     if (count == 0 || count > s->max_pairs || count >= s->max_frames || base_frame >= s->max_frames)
@@ -1373,7 +1381,7 @@ static int apply_chain_impl(rbf_stream* s, uint32_t base_frame, uint32_t count, 
             return set_err(c, RBF_ERR_INVALID, "pair %llu: motion vector component %d is outside [-%d, %d]",
                            (unsigned long long)(i / (field_bytes / count)), (int)fields[i], MV_RANGE, MV_RANGE);
     const uint64_t vbytes = value_offsets[count];
-    if (vbytes && !values) return set_err(c, RBF_ERR_INVALID, "rbf_stream_apply_chain: values is NULL");
+    if (vbytes && !values && !d_values) return set_err(c, RBF_ERR_INVALID, "rbf_stream_apply_chain: values is NULL");
     CK(c, cudaSetDevice(c->device));
     const uint32_t ntiles = (uint32_t)((s->npix + AP_TILE_PX - 1) / AP_TILE_PX);
     void *d_vals, *d_small, *d_pfx;
@@ -1382,12 +1390,13 @@ static int apply_chain_impl(rbf_stream* s, uint32_t base_frame, uint32_t count, 
     const size_t off_bytes = 8 * ((size_t)count + 1), flag_bytes = modes ? count : 0;
     const size_t res_at = align_up(off_bytes + flag_bytes + field_bytes, 16);
     const size_t small = res_at + 4 * ((size_t)count + 1) + (field_bytes ? 4 * (size_t)count : 0);   // + the runs' first_bad words
-    if ((rc = scratch_get(c, kScrValues, (size_t)vbytes + 256, &d_vals)) || (rc = scratch_get(c, kScrChainSmall, small, &d_small)) ||
+    d_vals = (void*)d_values;
+    if ((!d_values && (rc = scratch_get(c, kScrValues, (size_t)vbytes + 256, &d_vals))) || (rc = scratch_get(c, kScrChainSmall, small, &d_small)) ||
         (rc = scratch_get(c, kScrChainTiles, 4 * (size_t)count * ntiles, &d_pfx)))
         return rc;
     uint64_t* d_off = (uint64_t*)d_small;
     uint32_t* d_res = (uint32_t*)((uint8_t*)d_small + res_at);   // [0] first_bad, [1 + i] totals
-    if (vbytes) { CK(c, cudaMemcpyAsync(d_vals, values, (size_t)vbytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)vbytes; }
+    if (vbytes && !d_values) { CK(c, cudaMemcpyAsync(d_vals, values, (size_t)vbytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)vbytes; }
     if (modes) {
         std::vector<uint8_t> head(off_bytes + flag_bytes + field_bytes);
         memcpy(head.data(), value_offsets, off_bytes);
@@ -1584,8 +1593,7 @@ static int zlib_batch(rbf_ctx* c, uint32_t count, const void* const* srcs, const
             const Ref& r = refs[i];
             const uint32_t size = h_small[i];
             if (r.first) { offsets[r.buf] = pos; pos += 2; s1 = 1; s2 = 0; }
-            s2 = (uint32_t)((s2 + (uint64_t)r.len * s1 + h_small[W + 2 * i + 1]) % 65521u);
-            s1 = (uint32_t)((s1 + h_small[W + 2 * i]) % 65521u);
+            adler_combine(s1, s2, r.len, h_small[W + 2 * i], h_small[W + 2 * i + 1]);
             DeflateCopy cp;
             cp.src = (const uint8_t*)d_out + (size_t)i * region;
             cp.dst = pos - wave_start;
@@ -1630,6 +1638,222 @@ extern "C" int rbf_stream_zlib_changed(rbf_stream* s, uint32_t pairs, uint8_t* o
     std::vector<uint64_t> lens(pairs);
     for (uint32_t i = 0; i < pairs; i++) { srcs[i] = d_vals + voff[i]; lens[i] = voff[i + 1] - voff[i]; }
     return zlib_batch(c, pairs, srcs.data(), lens.data(), true, out_host, out_capacity, out_offsets);   // same stream: after the gather
+}
+
+// ------------------------------------------------------------------------------------------
+// inflate of the streams the device coder writes (rbf_inflate.cuh)
+// ------------------------------------------------------------------------------------------
+extern "C" int rbf_inflate_segment(const uint8_t* in, uint64_t avail, uint8_t* out, uint32_t* status, uint64_t* consumed,
+                                   uint32_t* produced, uint32_t* s1, uint32_t* s2) {
+    if ((!in && avail) || !out || !status || !consumed || !produced || !s1 || !s2)
+        return set_err(nullptr, RBF_ERR_INVALID, "rbf_inflate_segment: NULL");
+    InflateSegResult r;
+    inflate_segment_host(in, avail, out, &r);
+    *status = r.status; *consumed = r.consumed; *produced = r.produced; *s1 = r.adler & 0xffffu; *s2 = r.adler >> 16;
+    return RBF_OK;
+}
+
+// What inflate_streams leaves for inflate_place: per stream, its segments' slots in order and its inflated length; ok[i] == 0
+// for a stream the device declined (not in the layout, a segment refused on the chain, a bad trailer, more candidates than its
+// bound allows, or more output than its bound)
+struct InflateRun {
+    std::vector<std::vector<uint32_t>> chain;
+    std::vector<uint32_t> produced;     // per slot
+    std::vector<uint64_t> full;
+    std::vector<uint8_t> ok;
+    uint8_t* d_slots = nullptr;
+};
+
+// Host streams in: one H2D copy of each stream's bytes, k_inflate_scan, one sync for the candidate counts, k_inflate_segments
+// over every candidate, one sync for the results, and the chains resolved here.
+static int inflate_streams(rbf_ctx* c, uint32_t count, const void* const* srcs, const uint64_t* lens, const uint64_t* bounds,
+                           InflateRun& R) {
+    R.chain.assign(count, {}); R.full.assign(count, 0); R.ok.assign(count, 0); R.produced.clear();
+    std::vector<uint64_t> base(count, 0), cand0(count, 0), cap(count, 0);
+    std::vector<InflateScanJob> jobs;
+    uint64_t in_bytes = 0, ncand = 0;
+    for (uint32_t i = 0; i < count; i++) {
+        const uint8_t* p = (const uint8_t*)srcs[i];
+        if (!p || lens[i] < 8 || lens[i] > 0xfffffff0ull || p[0] != 0x78 || p[1] != 0x9c) continue;
+        const uint64_t by_bound = 2 * ((bounds[i] + kDeflateSeg - 1) / kDeflateSeg) + 8, by_len = lens[i] / 4 + 2;
+        cap[i] = by_bound < by_len ? by_bound : by_len;                // no more starts than 00 00 FF FF fits in the stream
+        base[i] = in_bytes; cand0[i] = ncand;
+        in_bytes += align_up(lens[i], 16); ncand += cap[i];
+        for (uint64_t q = 2; q < lens[i] - 6; q += kInflateScanChunk) {   // starts below the 6-byte trailer
+            const uint64_t e = q + kInflateScanChunk < lens[i] - 6 ? q + kInflateScanChunk : lens[i] - 6;
+            InflateScanJob J;
+            J.base = base[i]; J.begin = (uint32_t)q; J.end = (uint32_t)e; J.stream = i; J.cand0 = (uint32_t)cand0[i]; J.cap = (uint32_t)cap[i]; J.pad = 0;
+            jobs.push_back(J);
+        }
+        R.ok[i] = 1;
+    }
+    if (ncand > 0xffffffffull) return set_err(c, RBF_ERR_INVALID, "zlib inflate: %llu candidate starts in one call", (unsigned long long)ncand);
+    if (in_bytes == 0) return RBF_OK;
+    // small: counts[count] | cand[ncand] | start[ncand] | slot_stream[ncand] | streams[count] | jobs | err
+    const size_t o_cand = align_up(4 * (size_t)count, 16), o_start = align_up(o_cand + 4 * ncand, 16);
+    const size_t o_ss = align_up(o_start + 4 * ncand, 16), o_st = align_up(o_ss + 4 * ncand, 16);
+    const size_t o_jobs = align_up(o_st + sizeof(InflateStream) * count, 16), o_err = align_up(o_jobs + sizeof(InflateScanJob) * jobs.size(), 16);
+    void *d_in, *d_small;
+    int rc;
+    if ((rc = scratch_get(c, kScrInflateIn, in_bytes, &d_in)) || (rc = scratch_get(c, kScrInflateSmall, o_err + 16, &d_small))) return rc;
+    uint8_t* sm = (uint8_t*)d_small;
+    uint32_t* d_counts = (uint32_t*)sm;
+    for (uint32_t i = 0; i < count; i++)
+        if (R.ok[i]) { CK(c, cudaMemcpyAsync((uint8_t*)d_in + base[i], srcs[i], lens[i], cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)lens[i]; }
+    CK(c, cudaMemsetAsync(d_counts, 0, 4 * (size_t)count, c->st));
+    CK(c, cudaMemcpyAsync(sm + o_jobs, jobs.data(), sizeof(InflateScanJob) * jobs.size(), cudaMemcpyHostToDevice, c->st));
+    CK(c, launch_inflate_scan(c->L, (const InflateScanJob*)(sm + o_jobs), (int)jobs.size(), (const uint8_t*)d_in, d_counts,
+                              (uint32_t*)(sm + o_cand), c->st));
+    std::vector<uint32_t> counts(count);
+    CK(c, cudaMemcpyAsync(counts.data(), d_counts, 4 * (size_t)count, cudaMemcpyDeviceToHost, c->st));
+    c->d2h += 4 * (int64_t)count;
+    CK(c, cudaStreamSynchronize(c->st));
+    std::vector<InflateStream> streams(count);
+    std::vector<uint32_t> slot_stream;
+    for (uint32_t i = 0; i < count; i++) {
+        if (!R.ok[i]) continue;
+        if (counts[i] > cap[i]) { R.ok[i] = 0; continue; }
+        streams[i].base = base[i]; streams[i].len = lens[i]; streams[i].cand0 = (uint32_t)cand0[i]; streams[i].slot0 = (uint32_t)slot_stream.size();
+        slot_stream.insert(slot_stream.end(), counts[i], i);
+    }
+    const uint32_t nslots = (uint32_t)slot_stream.size();
+    std::vector<InflateSegResult> res(nslots);
+    std::vector<uint32_t> start(nslots);
+    if (nslots) {
+        void *d_slots, *d_res;
+        if ((rc = scratch_get(c, kScrInflateSlots, (size_t)nslots * kDeflateSeg, &d_slots)) ||
+            (rc = scratch_get(c, kScrInflateRes, sizeof(InflateSegResult) * (size_t)nslots, &d_res)))
+            return rc;
+        R.d_slots = (uint8_t*)d_slots;
+        CK(c, cudaMemcpyAsync(sm + o_ss, slot_stream.data(), 4 * (size_t)nslots, cudaMemcpyHostToDevice, c->st));
+        CK(c, cudaMemcpyAsync(sm + o_st, streams.data(), sizeof(InflateStream) * count, cudaMemcpyHostToDevice, c->st));
+        CK(c, launch_inflate_segments(c->L, (const uint32_t*)(sm + o_ss), (const InflateStream*)(sm + o_st), (int)nslots,
+                                      (const uint8_t*)d_in, (const uint32_t*)(sm + o_cand), R.d_slots, (InflateSegResult*)d_res,
+                                      (uint32_t*)(sm + o_start), c->st));
+        CK(c, cudaMemcpyAsync(res.data(), d_res, sizeof(InflateSegResult) * (size_t)nslots, cudaMemcpyDeviceToHost, c->st));
+        CK(c, cudaMemcpyAsync(start.data(), sm + o_start, 4 * (size_t)nslots, cudaMemcpyDeviceToHost, c->st));
+        c->d2h += (int64_t)(sizeof(InflateSegResult) + 4) * nslots;
+        CK(c, cudaStreamSynchronize(c->st));
+    }
+    R.produced.resize(nslots);
+    for (uint32_t k = 0; k < nslots; k++) R.produced[k] = res[k].produced;
+    // the chains: from offset 2 through each accepted segment's end, every segment but the last 64 KiB of output, to the trailer
+    std::vector<std::pair<uint32_t, uint32_t>> at;                     // (start, slot) of one stream, sorted
+    for (uint32_t i = 0; i < count; i++) {
+        if (!R.ok[i]) continue;
+        const uint8_t* p = (const uint8_t*)srcs[i];
+        const uint64_t end = lens[i] - 6;
+        at.clear();
+        for (uint32_t k = streams[i].slot0; k < streams[i].slot0 + counts[i]; k++) at.push_back({start[k], k});
+        std::sort(at.begin(), at.end());
+        uint64_t pos = 2, total = 0;
+        uint32_t s1 = 1, s2 = 0;
+        bool good = true;
+        std::vector<uint32_t>& chain = R.chain[i];
+        while (good && pos < end) {
+            auto it = std::lower_bound(at.begin(), at.end(), std::make_pair((uint32_t)pos, 0u));
+            good = it != at.end() && it->first == pos && res[it->second].status == kInflateOk &&
+                   (chain.empty() || res[chain.back()].produced == kDeflateSeg);
+            if (!good) break;
+            const InflateSegResult& r = res[it->second];
+            adler_combine(s1, s2, r.produced, r.adler & 0xffffu, r.adler >> 16);
+            total += r.produced;
+            pos += r.consumed;
+            chain.push_back(it->second);
+        }
+        const uint32_t trailer = (uint32_t)p[end + 2] << 24 | (uint32_t)p[end + 3] << 16 | (uint32_t)p[end + 4] << 8 | p[end + 5];
+        good = good && pos == end && p[end] == 0x03 && p[end + 1] == 0x00 && trailer == (s2 << 16 | s1) && total <= bounds[i];
+        if (!good) { R.ok[i] = 0; chain.clear(); continue; }
+        R.full[i] = total;
+    }
+    return RBF_OK;
+}
+
+// Copies each accepted stream's segments from their slots to d_dst + dst_off[i] (k_deflate_concat without header or trailer)
+static int inflate_place(rbf_ctx* c, const InflateRun& R, const uint64_t* dst_off, uint8_t* d_dst, uint64_t cap) {
+    std::vector<DeflateCopy> copies;
+    for (size_t i = 0; i < R.chain.size(); i++) {
+        uint64_t o = dst_off[i];
+        for (uint32_t k : R.chain[i]) {
+            DeflateCopy cp;
+            cp.src = R.d_slots + (size_t)k * kDeflateSeg; cp.dst = o; cp.len = R.produced[k]; cp.flags = cp.adler = cp.pad = 0;
+            copies.push_back(cp);
+            o += R.produced[k];
+        }
+    }
+    if (copies.empty()) return RBF_OK;
+    void* d_jobs;
+    if (int rc = scratch_get(c, kScrInflateRes, sizeof(DeflateCopy) * copies.size() + 16, &d_jobs)) return rc;   // the results are read
+    uint32_t* d_err = (uint32_t*)((uint8_t*)d_jobs + sizeof(DeflateCopy) * copies.size());
+    CK(c, cudaMemsetAsync(d_err, 0, 4, c->st));
+    CK(c, cudaMemcpyAsync(d_jobs, copies.data(), sizeof(DeflateCopy) * copies.size(), cudaMemcpyHostToDevice, c->st));
+    CK(c, launch_deflate_concat(c->L, (const DeflateCopy*)d_jobs, (int)copies.size(), d_dst, cap, d_err, c->st));
+    uint32_t err = 0;
+    CK(c, cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, c->st));
+    c->d2h += 4;
+    CK(c, cudaStreamSynchronize(c->st));
+    if (err) return set_err(c, RBF_ERR_STATE, "zlib inflate: a placed segment overran the output");
+    return RBF_OK;
+}
+
+extern "C" int rbf_zlib_decompress_batch(rbf_ctx* c, uint32_t count, const void* const* srcs, const uint64_t* lens, const uint64_t* bounds,
+                                         uint8_t* out_host, uint64_t out_capacity, uint64_t* out_offsets, uint8_t* on_device) {
+    if (!c || !out_offsets || (count && (!srcs || !lens || !bounds || !on_device)))
+        return set_err(c, RBF_ERR_INVALID, "rbf_zlib_decompress_batch: NULL");
+    CK(c, cudaSetDevice(c->device));
+    InflateRun R;
+    if (int rc = inflate_streams(c, count, srcs, lens, bounds, R)) return rc;
+    out_offsets[0] = 0;
+    for (uint32_t i = 0; i < count; i++) {
+        if (R.ok[i] && R.full[i] > out_capacity - out_offsets[i]) { R.ok[i] = 0; R.full[i] = 0; R.chain[i].clear(); }   // does not fit
+        on_device[i] = R.ok[i];
+        out_offsets[i + 1] = out_offsets[i] + R.full[i];
+    }
+    const uint64_t total = out_offsets[count];
+    if (total == 0) return RBF_OK;
+    if (!out_host) return set_err(c, RBF_ERR_INVALID, "rbf_zlib_decompress_batch: out_host is NULL");
+    void* d_out;
+    if (int rc = scratch_get(c, kScrInflateOut, total, &d_out)) return rc;
+    if (int rc = inflate_place(c, R, out_offsets, (uint8_t*)d_out, total)) return rc;
+    CK(c, cudaMemcpyAsync(out_host, d_out, total, cudaMemcpyDeviceToHost, c->st));
+    c->d2h += (int64_t)total;
+    CK(c, cudaStreamSynchronize(c->st));
+    return RBF_OK;
+}
+
+extern "C" int rbf_stream_inflate_values(rbf_stream* s, uint32_t count, const void* const* srcs, const uint64_t* lens,
+                                         const uint64_t* bounds, uint64_t* out_lens, uint8_t* on_device) {
+    if (!s || (count && (!srcs || !lens || !bounds || !out_lens || !on_device)))
+        return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_inflate_values: NULL");
+    rbf_ctx* c = s->c;
+    CK(c, cudaSetDevice(c->device));
+    s->inflated_bytes = 0;
+    InflateRun R;
+    if (int rc = inflate_streams(c, count, srcs, lens, bounds, R)) return rc;
+    std::vector<uint64_t> off(count + 1, 0);
+    for (uint32_t i = 0; i < count; i++) { on_device[i] = R.ok[i]; out_lens[i] = R.full[i]; off[i + 1] = off[i] + R.full[i]; }
+    const uint64_t total = off[count];
+    if (total + 256 > s->inflated_cap) {
+        if (s->d_inflated) CK(c, cudaFree(s->d_inflated));
+        s->d_inflated = nullptr; s->inflated_cap = 0;
+        const size_t nb = align_up((size_t)total + (total >> 2) + 256, 256);
+        CK(c, cudaMalloc((void**)&s->d_inflated, nb));
+        s->inflated_cap = nb;
+    }
+    if (int rc = inflate_place(c, R, off.data(), s->d_inflated, total)) return rc;
+    s->inflated_bytes = total;
+    return RBF_OK;
+}
+
+extern "C" int rbf_stream_apply_chain_inflated(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint64_t* value_offsets,
+                                               const uint8_t* modes, const int8_t* fields, uint64_t* applied_out) {
+    if (!s || !value_offsets || !modes) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_apply_chain_inflated: NULL");
+    if (count && value_offsets[count] > s->inflated_bytes)
+        return set_err(s->c, RBF_ERR_INVALID, "rbf_stream_apply_chain_inflated: %llu value bytes, %llu inflated",
+                       (unsigned long long)value_offsets[count], (unsigned long long)s->inflated_bytes);
+    const int rc = apply_chain_impl(s, base_frame, count, nullptr, value_offsets, modes, 2, fields, applied_out, s->d_inflated);
+    s->inflated_bytes = 0;
+    return rc;
 }
 
 // ------------------------------------------------------------------------------------------

@@ -10,6 +10,7 @@
 //   K5  k_motion_search  16 x 16 block motion search, +-16 px (value_coding "motion")
 //       k_apply_motion   a motion-compensated residual pair of a decoded group
 //   N4  k_deflate_segments / k_deflate_concat   zlib streams of host or device buffers (rbf_deflate.cuh)
+//       k_inflate_scan / k_inflate_segments     inflate of those streams, segment by segment (rbf_inflate.cuh)
 //
 // The Bloom bit array of the frame being queried is staged into shared memory with
 // cp.async.bulk (TMA bulk copy, mbarrier complete_tx); whatever exceeds the 227 KB of a
@@ -111,6 +112,7 @@ __device__ __forceinline__ void or_bits128(uint32_t* __restrict__ W, uint64_t bi
 #include "rbf_k3b_witness.cuh"
 #include "rbf_aux_kernels.cuh"
 #include "rbf_deflate.cuh"
+#include "rbf_inflate.cuh"
 #include "rbf_k4c_apply.cuh"
 #include "rbf_motion.cuh"
 
@@ -618,6 +620,23 @@ cudaError_t launch_deflate_concat(LaunchCfg& L, const DeflateCopy* d_jobs, int c
 int deflate_code_lengths_host(const uint32_t* freqs, uint32_t nsym, uint32_t max_bits, uint8_t* lengths) {
     HuffScratch S;
     return deflate_code_lengths(freqs, nsym, max_bits, lengths, &S);
+}
+cudaError_t launch_inflate_scan(LaunchCfg& L, const InflateScanJob* d_jobs, int count, const uint8_t* d_in, uint32_t* d_counts,
+                                uint32_t* d_cand, cudaStream_t st) {
+    if (count <= 0) return cudaSuccess;
+    k_inflate_scan<<<count, 256, 0, st>>>(d_jobs, d_in, d_counts, d_cand);
+    return counted(L);
+}
+cudaError_t launch_inflate_segments(LaunchCfg& L, const uint32_t* d_slot_stream, const InflateStream* d_streams, int nslots,
+                                    const uint8_t* d_in, const uint32_t* d_cand, uint8_t* d_slots, InflateSegResult* d_res,
+                                    uint32_t* d_start, cudaStream_t st) {
+    if (nslots <= 0) return cudaSuccess;
+    k_inflate_segments<<<nslots, 32, 0, st>>>(d_slot_stream, d_streams, d_in, d_cand, d_slots, d_res, d_start);
+    return counted(L);
+}
+void inflate_segment_host(const uint8_t* in, uint64_t avail, uint8_t* out, InflateSegResult* res) {
+    InflateScratch S;
+    inflate_segment(in, avail, out, &S, res);
 }
 
 }  // namespace rbf

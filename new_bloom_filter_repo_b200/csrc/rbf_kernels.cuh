@@ -96,6 +96,28 @@ struct DeflateCopy {
     uint32_t pad;
 };
 
+// inflate of that layout (rbf_inflate.cuh): candidate segment starts of each stream, each inflated into its own kDeflateSeg slot
+enum : uint32_t {
+    kInflateOk = 0, kInflateTruncated, kInflateFinal, kInflateBlockType, kInflateStoredLen, kInflateHeader, kInflateCodeLengths,
+    kInflateRepeat, kInflateNoEnd, kInflateLitCode, kInflateDistCode, kInflateBadSymbol, kInflateBadDistance, kInflateTooFar,
+    kInflateOutputFull,
+};
+static constexpr uint32_t kInflateScanChunk = 8192;    // candidate positions per k_inflate_scan job
+struct InflateSegResult { uint32_t status, consumed, produced, adler; };   // adler: s2 << 16 | s1 of the segment, from (0, 0)
+struct InflateScanJob {
+    uint64_t base;        // the stream's first byte in the input buffer
+    uint32_t begin, end;  // positions [begin, end) of the stream this job scans
+    uint32_t stream, cand0, cap, pad;   // the stream's candidates go to cand[cand0 .. cand0 + cap)
+};
+struct InflateStream {
+    uint64_t base, len;
+    uint32_t cand0, slot0;   // its candidates in cand[] and its first slot
+};
+// Adler-32 (s1, s2) of a prefix followed by a part of len bytes whose own sums from (0, 0) are (a1, a2)
+__host__ __device__ __forceinline__ void adler_combine(uint32_t& s1, uint32_t& s2, uint64_t len, uint32_t a1, uint32_t a2) {
+    s2 = (uint32_t)((s2 + (len % 65521u) * s1 + a2) % 65521u);
+    s1 = (uint32_t)((s1 + a1) % 65521u);
+}
 
 // What the launchers read from the context (rbf_set_option), and its kernel counter: every launcher adds the kernels it enqueued.
 struct LaunchCfg {
@@ -181,6 +203,12 @@ cudaError_t launch_deflate_segments(LaunchCfg& L, const DeflateSeg* d_segs, int 
 cudaError_t launch_deflate_concat(LaunchCfg& L, const DeflateCopy* d_jobs, int count, uint8_t* d_dst, uint64_t cap, uint32_t* d_err,
                                   cudaStream_t st);
 int deflate_code_lengths_host(const uint32_t* freqs, uint32_t nsym, uint32_t max_bits, uint8_t* lengths);
+cudaError_t launch_inflate_scan(LaunchCfg& L, const InflateScanJob* d_jobs, int count, const uint8_t* d_in, uint32_t* d_counts,
+                                uint32_t* d_cand, cudaStream_t st);
+cudaError_t launch_inflate_segments(LaunchCfg& L, const uint32_t* d_slot_stream, const InflateStream* d_streams, int nslots,
+                                    const uint8_t* d_in, const uint32_t* d_cand, uint8_t* d_slots, InflateSegResult* d_res,
+                                    uint32_t* d_start, cudaStream_t st);
+void inflate_segment_host(const uint8_t* in, uint64_t avail, uint8_t* out, InflateSegResult* res);
 
 int query_max_smem_bytes();
 

@@ -2,7 +2,8 @@
 Keyframe codec + YUV frame wrapper: host glue kept byte-compatible with the reference's
 fixed_video_compressor.py (FixedVideoCompressor fvc:15-334) so that keyframe payloads written by
 either implementation decode with the other.  zlib entropy coding is CPU work outside the
-accelerated path (SURVEY.md section 8f, N4); nothing here touches the GPU.
+accelerated path (SURVEY.md section 8f, N4); nothing here touches the GPU (decompress_video inflates keyframe blobs of the
+device coder on the GPU and builds the frame with build_frame).
 """
 from __future__ import annotations
 
@@ -96,10 +97,35 @@ class FixedVideoCompressor:
         return lambda: assemble_keyframe(frame, [f.result() for f in futs])
 
     def decompress_frame(self, data: bytes):                                     # fvc:76-181
+        return self.build_frame(data, zlib.decompress)
+
+    @staticmethod
+    def keyframe_blobs(data: bytes):
+        """The layout parse of a keyframe payload: [(zlib blob, most bytes it may inflate to)] for the frame and, YUV frames,
+        the three planes, in payload order; the bounds are h w itemsize 4 for the frame and ph pw for a plane.  Raises
+        struct.error (or another exception) on a truncated layout, as decompress_frame would reach it."""
+        h, w, isz = struct.unpack_from("<III", data, 0)
+        (zlen,) = struct.unpack_from("<I", data, 12)
+        blobs = [(data[16:16 + zlen], h * w * isz * 4)]
+        pos = 16 + zlen
+        if not (pos < len(data) and data[pos] == 1):
+            return blobs
+        (flen,) = struct.unpack_from("<H", data, pos + 1)
+        pos += 3 + flen
+        for _ in range(3):
+            (zl,) = struct.unpack_from("<I", data, pos)
+            ph, pw = struct.unpack_from("<II", data, pos + 4 + zl)
+            blobs.append((data[pos + 4:pos + 4 + zl], ph * pw))
+            pos += 12 + zl
+        return blobs
+
+    def build_frame(self, data: bytes, inflate):
+        """decompress_frame with inflate(blob) in place of zlib.decompress: called for the frame blob, then for each plane blob,
+        at the points of the parse where decompress_frame inflates them."""
         h, w, isz = struct.unpack_from("<III", data, 0)
         (zlen,) = struct.unpack_from("<I", data, 12)
         pos = 16
-        raw = zlib.decompress(data[pos:pos + zlen])
+        raw = inflate(data[pos:pos + zlen])
         pos += zlen
         dtype = _DTYPES.get(isz, np.float32)
         gray = h * w * isz
@@ -118,7 +144,7 @@ class FixedVideoCompressor:
         for name in ("y_plane", "u_plane", "v_plane"):
             (zl,) = struct.unpack_from("<I", data, pos)
             pos += 4
-            plane_raw = zlib.decompress(data[pos:pos + zl])
+            plane_raw = inflate(data[pos:pos + zl])
             pos += zl
             ph, pw = struct.unpack_from("<II", data, pos)
             pos += 8

@@ -378,11 +378,12 @@ class _InterPayload:
 
 class _InterJob:
     """An inter frame on its way through decompress_video: the parsed payload (or its parse error) and its inflates."""
-    __slots__ = ("p", "err", "values", "mask", "field", "values_arr", "mask_arr", "field_arr", "l", "wlen")
+    __slots__ = ("p", "err", "values", "mask", "field", "values_arr", "mask_arr", "field_arr", "l", "wlen", "vlen", "vsize")
 
     def __init__(self):
         self.p = self.err = self.values = self.mask = self.field = self.values_arr = self.mask_arr = self.field_arr = None
-        self.l = self.wlen = 0
+        self.vlen = None                                     # bytes of the value stream inflated on the GPU (_inflate_group)
+        self.l = self.wlen = self.vsize = 0
 
 
 class ImprovedVideoCompressor:
@@ -687,7 +688,8 @@ class ImprovedVideoCompressor:
         except Exception as e:                               # re-raised in file order by _check_inter
             job.err = e
             return job
-        job.values = pool.submit(zlib.decompress, job.p.vz)
+        if bytes(job.p.vz[:2]) != deflate._DEVICE_HEADER:  # the device coder's streams are inflated per group on the GPU
+            job.values = pool.submit(zlib.decompress, job.p.vz)
         if job.p.vmode == 2:
             job.field = pool.submit(zlib.decompress, job.p.fz)
         if job.p.raw and not job.p.v1:
@@ -702,12 +704,19 @@ class ImprovedVideoCompressor:
             raise job.err
         p = job.p
         dtype = np.dtype(np.uint8 if p.isz == 1 else np.uint16)
-        job.values_arr = np.frombuffer(job.values.result(), dtype=dtype)[:p.vcount]
+        if job.vlen is None:                                 # (a stream left for the GPU that no group inflated: here)
+            raw = job.values.result() if job.values is not None else zlib.decompress(p.vz)
+            job.values_arr = np.frombuffer(raw, dtype=dtype)[:p.vcount]
+            job.vsize = job.values_arr.size
+        else:                                                # on the device: the same count, and numpy's error for a ragged length
+            if job.vlen % dtype.itemsize:
+                np.frombuffer(bytes(job.vlen % dtype.itemsize), dtype=dtype)
+            job.vsize = min(job.vlen // dtype.itemsize, p.vcount)
         exp_shape = (p.h, p.w, p.ch) if p.ch > 1 else (p.h, p.w)
         if pdata.shape != exp_shape or pdata.dtype != dtype:
             raise ValueError(f"inter frame {exp_shape}/{dtype} does not match the previous frame {pdata.shape}/{pdata.dtype}")
-        if job.values_arr.size != p.ones * p.ch:
-            raise ValueError(f"corrupt inter frame: {job.values_arr.size} changed values for {p.ones} changed pixels x {p.ch} channels")
+        if job.vsize != p.ones * p.ch:
+            raise ValueError(f"corrupt inter frame: {job.vsize} changed values for {p.ones} changed pixels x {p.ch} channels")
         if p.vmode == 2:
             nfield = 2 * ((p.h + 15) // 16) * ((p.w + 15) // 16)
             job.field_arr = np.frombuffer(job.field.result(), dtype=np.int8)
@@ -751,13 +760,34 @@ class ImprovedVideoCompressor:
                 raise IndexError("list index out of range")
             if ones[i] != j.p.ones:                          # the reference would silently return the base frame (ivc:882)
                 raise ValueError(f"corrupt inter frame: the decoded mask selects {int(ones[i])} pixels, the payload announces {j.p.ones}")
-        applied = st.apply_chain(base, [j.values_arr for j in group], residual=[j.p.vmode for j in group],
-                                 motion=[j.field_arr for j in group])
+        if group[0].vlen is not None:                        # the group's values are on the device (_inflate_group)
+            applied = st.apply_chain_inflated(base, [j.vsize * j.p.isz for j in group], [j.p.vmode for j in group],
+                                              motion=[j.field_arr for j in group])
+        else:
+            applied = st.apply_chain(base, [j.values_arr for j in group], residual=[j.p.vmode for j in group],
+                                     motion=[j.field_arr for j in group])
         if not np.array_equal(applied, ones):
             raise ValueError(f"corrupt inter frame: {applied.tolist()} pixels applied, {ones.tolist()} expected")
         return st.download_batch((base + 1) % st.max_frames, m)
 
-    def _decode_run(self, run: List["_InterJob"], prev, streams: Dict[tuple, FrameStream]) -> list:
+    @staticmethod
+    def _inflate_group(st: FrameStream, jobs: List["_InterJob"], pool) -> None:
+        """The value streams of a group's payloads, when all are the device coder's, inflated on the GPU into `st` (job.vlen).  If
+        any is not, or the device declines one, every stream of the group is inflated on the host as before."""
+        parsed = [j for j in jobs if j.p is not None]
+        dev = [j for j in parsed if j.values is None]
+        if not dev:
+            return
+        if len(dev) == len(parsed):
+            lens, ok = st.inflate_values([j.p.vz for j in dev], [j.p.vcount * j.p.isz for j in dev])
+            if ok.all():
+                for j, n in zip(dev, lens):
+                    j.vlen = int(n)
+                return
+        for j in dev:
+            j.values = pool.submit(zlib.decompress, j.p.vz)
+
+    def _decode_run(self, run: List["_InterJob"], prev, streams: Dict[tuple, FrameStream], pool) -> list:
         """The frames of a run of consecutive inter payloads that follows `prev`, in groups of batch_size.  The run's base frame is
         uploaded once; each group chains from the previous group's last frame, which stays on the device."""
         pdata = np.ascontiguousarray(_frame_data(prev))
@@ -765,6 +795,10 @@ class ImprovedVideoCompressor:
         out, st, base = [], None, 0
         for g0 in range(0, len(run), group_size):
             group, err = [], None
+            if any(j.p is not None and j.values is None for j in run[g0:g0 + group_size]):
+                if st is None:
+                    st = self._run_stream(pdata, group_size, streams)
+                self._inflate_group(st, run[g0:g0 + group_size], pool)
             for job in run[g0:g0 + group_size]:
                 try:
                     self._check_inter(job, pdata)
@@ -774,13 +808,7 @@ class ImprovedVideoCompressor:
                 group.append(job)
             if group:
                 if st is None:
-                    ch = pdata.shape[2] if pdata.ndim == 3 else 1
-                    key = (pdata.shape, pdata.dtype.str)
-                    st = streams.get(key)
-                    if st is None:
-                        st = streams[key] = FrameStream(pdata.shape[0], pdata.shape[1], ch, pdata.dtype, max_frames=group_size + 1,
-                                                        max_pairs=group_size, k1_only=True)
-                    st.upload(pdata, first=0)
+                    st = self._run_stream(pdata, group_size, streams)
                 dec = self._decode_group(st, base, group)
                 base = (base + len(group)) % st.max_frames
                 out += [YUVFrame(f) if hasattr(prev, "yuv_info") else f for f in dec]
@@ -788,10 +816,46 @@ class ImprovedVideoCompressor:
                 raise err
         return out
 
+    @staticmethod
+    def _run_stream(pdata: np.ndarray, group_size: int, streams: Dict[tuple, FrameStream]) -> FrameStream:
+        """The device store a run decodes in (one per frame shape and dtype), with the run's base frame uploaded to slot 0."""
+        ch = pdata.shape[2] if pdata.ndim == 3 else 1
+        key = (pdata.shape, pdata.dtype.str)
+        st = streams.get(key)
+        if st is None:
+            st = streams[key] = FrameStream(pdata.shape[0], pdata.shape[1], ch, pdata.dtype, max_frames=group_size + 1,
+                                            max_pairs=group_size, k1_only=True)
+        st.upload(pdata, first=0)
+        return st
+
+    def _start_key(self, payload: bytes, pool):
+        """A keyframe's decode: its blobs inflated on the GPU in one batch when all are the device coder's (then built with
+        build_frame when decoding reaches the frame), else decompress_frame in `pool`.  Anything the GPU route raises sends the
+        frame to decompress_frame, which raises what it always did."""
+        try:
+            blobs = self.compressor.keyframe_blobs(payload)
+        except Exception:
+            blobs = None
+        if not blobs or any(bytes(b[:2]) != deflate._DEVICE_HEADER for b, _ in blobs):
+            return pool.submit(self.compressor.decompress_frame, payload)
+        comp = self.compressor
+
+        class _Job:
+            @staticmethod
+            def result():
+                try:
+                    raws = iter(deflate.decompress_many([b for b, _ in blobs], [n for _, n in blobs]))
+                    return comp.build_frame(payload, lambda _blob: next(raws))
+                except Exception:
+                    return comp.decompress_frame(payload)
+        return _Job()
+
     def decompress_video(self, input_path: str = None, output_path: Optional[str] = None,
                          compressed_frames: List[bytes] = None, metadata: Dict = None) -> List[np.ndarray]:
-        """ivc:452-504.  Every zlib stream (keyframe blobs, changed values, raw masks) is inflated in a pool of num_threads; each
-        run of inter frames is rebuilt on the GPU in groups of batch_size (_decode_run)."""
+        """ivc:452-504.  Each run of inter frames is rebuilt on the GPU in groups of batch_size (_decode_run).  zlib streams of the
+        GPU entropy coder (78 9C: keyframe blobs, changed values) are inflated on the GPU -- a group's value streams straight into
+        the buffer its reconstruction reads; every other zlib stream (CPU zlib's 78 DA, raw masks, motion fields), and any stream
+        the GPU declines, is inflated with zlib.decompress in a pool of num_threads."""
         if input_path and os.path.exists(input_path):                              # ivc:471-485
             with open(input_path, "rb") as fh:
                 magic = fh.read(4)
@@ -809,8 +873,8 @@ class ImprovedVideoCompressor:
         streams: Dict[tuple, FrameStream] = {}
         pool = ThreadPoolExecutor(self.num_threads)
         try:
-            jobs = [self._start_inter(c, pool) if c[:len(_INTER_TAG)] in _INTER_TAGS
-                    else pool.submit(self.compressor.decompress_frame, c) for c in compressed_frames]
+            jobs = [self._start_inter(c, pool) if c[:len(_INTER_TAG)] in _INTER_TAGS else self._start_key(c, pool)
+                    for c in compressed_frames]
             i = 0
             while i < len(jobs):
                 if not isinstance(jobs[i], _InterJob):
@@ -822,7 +886,7 @@ class ImprovedVideoCompressor:
                 j = i
                 while j < len(jobs) and isinstance(jobs[j], _InterJob):
                     j += 1
-                frames += self._decode_run(jobs[i:j], frames[-1], streams)
+                frames += self._decode_run(jobs[i:j], frames[-1], streams, pool)
                 i = j
         finally:
             pool.shutdown(wait=True, cancel_futures=True)

@@ -243,15 +243,7 @@ class FrameStream:
             if flags.shape != (len(parts),):
                 raise ValueError("one residual flag per pair")
         if motion is not None and flags is not None and (flags == 2).any():
-            fields = np.zeros((len(parts),) + self.mv_shape + (2,), dtype=np.int8)
-            for i in np.flatnonzero(flags == 2):
-                f = motion[i] if i < len(motion) else None
-                if f is None:
-                    raise ValueError(f"pair {i} is a motion pair without a motion field")
-                f = np.asarray(f)
-                if f.dtype != np.int8 or f.size != fields[i].size:
-                    raise ValueError(f"pair {i}: a motion field is {fields[i].size} int8 values, not {f.size} {f.dtype}")
-                fields[i] = f.reshape(fields[i].shape)
+            fields = self._motion_fields(flags, motion)
             _cabi.check(_cabi.lib().rbf_stream_apply_chain_motion(self._h, int(base_frame), len(parts), _cabi.ptr(buf) if buf.size else None,
                                                                   _cabi.ptr(offs), _cabi.ptr(flags), _cabi.ptr(fields), _cabi.ptr(applied)),
                         _cabi.ctx())
@@ -259,6 +251,50 @@ class FrameStream:
         _cabi.check(_cabi.lib().rbf_stream_apply_chain_modes(self._h, int(base_frame), len(parts), _cabi.ptr(buf) if buf.size else None,
                                                              _cabi.ptr(offs), _cabi.ptr(flags) if flags is not None else None,
                                                              _cabi.ptr(applied)), _cabi.ctx())
+        return applied
+
+    def _motion_fields(self, flags: np.ndarray, motion) -> np.ndarray:
+        """The [count, by, bx, 2] int8 fields of apply_chain's mode-2 pairs (zero for the others)."""
+        fields = np.zeros((flags.size,) + self.mv_shape + (2,), dtype=np.int8)
+        for i in np.flatnonzero(flags == 2):
+            f = motion[i] if i < len(motion) else None
+            if f is None:
+                raise ValueError(f"pair {i} is a motion pair without a motion field")
+            f = np.asarray(f)
+            if f.dtype != np.int8 or f.size != fields[i].size:
+                raise ValueError(f"pair {i}: a motion field is {fields[i].size} int8 values, not {f.size} {f.dtype}")
+            fields[i] = f.reshape(fields[i].shape)
+        return fields
+
+    def inflate_values(self, streams: Sequence, bounds: Sequence[int]):
+        """The zlib value streams of a group inflated on the GPU into the stream's value buffer, for apply_chain_inflated.
+        bounds[i]: the most stream i may hold (its value count x sample bytes).  -> (inflated bytes uint64[n], on_device bool[n]);
+        a declined stream (not the device coder's layout, or larger than its bound) has on_device False and 0 bytes."""
+        views = [np.frombuffer(memoryview(s).cast("B"), dtype=np.uint8) for s in streams]
+        n = len(views)
+        lens = np.array([v.size for v in views], dtype=np.uint64)
+        bnd = np.ascontiguousarray(np.asarray(bounds, dtype=np.uint64))
+        srcs = (C.c_void_p * n)(*[v.ctypes.data if v.size else None for v in views])
+        out = np.zeros(n, dtype=np.uint64)
+        ok = np.zeros(n, dtype=np.uint8)
+        _cabi.check(_cabi.lib().rbf_stream_inflate_values(self._h, n, srcs, _cabi.ptr(lens), _cabi.ptr(bnd), _cabi.ptr(out), _cabi.ptr(ok)),
+                    _cabi.ctx())
+        return out, ok.astype(bool)
+
+    def apply_chain_inflated(self, base_frame: int, nbytes: Sequence[int], residual: Sequence[int],
+                             motion: Optional[Sequence[Optional[np.ndarray]]] = None) -> np.ndarray:
+        """apply_chain with pair i's values the first nbytes[i] bytes of the i-th stream the last inflate_values placed (every one
+        of them inflated on the device, in order): the values never cross PCIe."""
+        offs = np.zeros(len(nbytes) + 1, dtype=np.uint64)
+        offs[1:] = np.cumsum(np.asarray(nbytes, dtype=np.uint64))
+        flags = np.ascontiguousarray(np.asarray(residual, dtype=np.uint8))
+        if flags.shape != (len(nbytes),):
+            raise ValueError("one value mode per pair")
+        fields = self._motion_fields(flags, motion) if motion is not None and (flags == 2).any() else None
+        applied = np.zeros(len(nbytes), dtype=np.uint64)
+        _cabi.check(_cabi.lib().rbf_stream_apply_chain_inflated(self._h, int(base_frame), len(nbytes), _cabi.ptr(offs), _cabi.ptr(flags),
+                                                                _cabi.ptr(fields) if fields is not None else None, _cabi.ptr(applied)),
+                    _cabi.ctx())
         return applied
 
     def download_batch(self, first: int, count: int) -> np.ndarray:

@@ -52,10 +52,10 @@ def per_frame_decode(comp, payloads):
 
 class StageTimer:
     """Device-event time (rbf_timer_start / rbf_timer_stop_ms on the context's stream) of FrameStream.decode_masks and
-    FrameStream.apply_chain, per call."""
+    FrameStream.apply_chain -- or, for GPU-coded files, inflate_values and apply_chain_inflated -- per call."""
 
     def __init__(self):
-        self.ms = {"decode_masks": [], "apply_chain": []}
+        self.ms = {"inflate_values": [], "decode_masks": [], "apply_chain": [], "apply_chain_inflated": []}
         self._orig = {}
 
     def __enter__(self):
@@ -116,7 +116,9 @@ def run(h, w, coder, runs=3):
             "decompress_fps": [round(30 / t, 2) for t in t_new], "per_frame_route_fps": [round(30 / t, 2) for t in t_old],
             "identical_frames": True,
             "decode_masks_ms_per_group": [round(x, 3) for x in tm.ms["decode_masks"]],
-            "apply_chain_ms_per_group": [round(x, 3) for x in tm.ms["apply_chain"]]}
+            "apply_chain_ms_per_group": [round(x, 3) for x in tm.ms["apply_chain"]],
+            "inflate_values_ms_per_group": [round(x, 3) for x in tm.ms["inflate_values"]],
+            "apply_chain_inflated_ms_per_group": [round(x, 3) for x in tm.ms["apply_chain_inflated"]]}
 
 
 if __name__ == "__main__":
