@@ -21,6 +21,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <mutex>
+
 #include "rbf_kernels.cuh"
 
 namespace rbf {
@@ -278,12 +280,18 @@ static cudaError_t launch_query2_t(LaunchCfg& L, const FrameJob* d_jobs, const u
     return counted(L);
 }
 
+// A kernel's dynamic shared memory limit (cudaFuncSetAttribute) is one value for the whole process, and the query sets it to what
+// each launch needs, which depends on l.  Contexts driven from different host threads must not interleave their set and launch: a
+// thread that lowers the limit in between makes the other's launch fail with "too many resources requested for launch".
+static std::mutex g_query_smem_attr;
+
 // variant: 0 per-lane kernel; 1 staged rings; 5 decade tiles (half-decade tiles for 2^23 < m <= 2^24, rings beyond); 6 half-decade
 // tiles for every m <= 2^24.  (2, 3 and 4 selected earlier kernels that were measured slower and removed; the values still
 // select the current default.)
 cudaError_t launch_query(LaunchCfg& L, const FrameJob* d_jobs, const uint32_t* d_cent_prefix, int F, uint32_t total_centuries,
                          uint32_t max_l_bits, cudaStream_t st) {
     if (F <= 0 || total_centuries == 0) return cudaSuccess;
+    std::lock_guard<std::mutex> attr_and_launch(g_query_smem_attr);
     int variant = L.query_variant, tile_warps = L.query_warps;
     if (tile_warps < 4 || tile_warps > Q4_WARPS) tile_warps = 0;                       // 0: the tile width's default
     int cap = L.query_smem_cap & ~15;

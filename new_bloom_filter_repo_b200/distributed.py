@@ -203,6 +203,12 @@ class ShardedStreamEncoder:
         self.dist = dist
         self.world, self.rank = dist.get_world_size(), dist.get_rank()
         self.total_pairs = int(total_frames) - 1
+        if self.total_pairs < self.world:
+            # a rank without a pair has no block to code (its stream would hold the halo frame alone) and would leave the other
+            # ranks waiting in the first collective; every rank sees the same arguments, so every rank raises here, before any
+            # collective and before any device allocation
+            raise ValueError("a stream of %d frames has %d frame pairs for %d ranks: every rank needs at least one pair"
+                             % (int(total_frames), max(self.total_pairs, 0), self.world))
         self.layout = shard_layout(self.total_pairs, self.rank, self.world)
         self.gather = gather
         self.stream = FrameStream(height, width, channels, dtype, max_frames=self.layout["frames"],

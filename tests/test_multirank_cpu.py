@@ -7,6 +7,7 @@ import subprocess
 import sys
 
 import numpy as np
+import pytest
 
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
 
@@ -41,3 +42,29 @@ def test_world_size_2_gloo(tmp_path):
         assert lay["slots"] == 15 and lay["frames"] == lay["pairs"] + 1 and lay["first_frame"] == lay["lo"] == o["lo"]
         assert [h[0] for h in o["headers"]] == list(range(pairs))
         assert [tuple(r) for r in o["rows"]] == [(h[1], h[0] - outs[h[1]]["lo"]) for h in o["headers"]]
+
+
+class _NoCollectives:
+    """A rank of `world` whose collectives must not be reached."""
+
+    def __init__(self, rank, world):
+        self.rank, self.world = rank, world
+
+    def get_rank(self):
+        return self.rank
+
+    def get_world_size(self):
+        return self.world
+
+    def __getattr__(self, name):
+        raise AssertionError("collective %s entered" % name)
+
+
+def test_sharded_encoder_needs_a_pair_per_rank():
+    """Fewer frame pairs than ranks: every rank, including those that would own a pair, raises ValueError in the constructor,
+    before any collective and before the library is touched (so this runs without a GPU)."""
+    from new_bloom_filter_repo_b200 import distributed as rdist
+    for world, total_frames in ((4, 3), (2, 2), (3, 1), (1, 1), (16, 16)):
+        for rank in range(world):
+            with pytest.raises(ValueError, match="every rank needs at least one pair"):
+                rdist.ShardedStreamEncoder(_NoCollectives(rank, world), 8, 8, 3, np.uint8, total_frames, max_l_bits=64)
