@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define RBF_ABI_VERSION 2
+#define RBF_ABI_VERSION 3
 
 typedef enum {
     RBF_OK = 0,
@@ -211,36 +211,34 @@ int rbf_stream_download(rbf_stream* s, uint32_t frame, void* host_out);
  *     The bit-array, witness and mask slots no longer hold an encode's outputs afterwards: fetch / gather / decode_verify
  *     refuse until the next rbf_stream_encode.
  * rbf_stream_apply_chain   VideoFrameCompressor._apply_frame_diff (ivc:849-909) along a chain: frame base_frame+1+i = frame
- *     base_frame+i with mask slot i applied (its set pixels replaced, in rank order, by the value bytes
- *     values[value_offsets[i], value_offsets[i+1])), i < count; one H2D copy of the values, one synchronisation.  Frame slots
- *     are taken modulo max_frames, so a chain may continue from the last frame of the previous one wherever it sits; count <
- *     max_frames.  ivc:882 per pair: pair i is applied only if its mask's popcount x pixel bytes equals its value bytes; the
- *     first pair that fails gets applied_out[i] = 0 and no frame from there on is written.  applied_out[i] = pixels applied.
- * rbf_stream_apply_chain_modes  rbf_stream_apply_chain with a coding per pair: residual[i] == 1 means pair i's values are
- *     residuals (what a gather with value_mode 1 returns), added to the selected pixels per sample mod 2^(8 sample_bytes) instead
- *     of replacing them; 0 means plain values.  residual may be NULL (every pair plain: rbf_stream_apply_chain itself); a flag
- *     other than 0 or 1 is RBF_ERR_INVALID.  The flags travel in the same H2D copy as the offsets; ivc:882, the first-bad-pair
- *     rule and slot wrap-around are the same for both kinds.
- * rbf_stream_apply_chain_motion  rbf_stream_apply_chain_modes with a third mode: modes[i] == 2 means pair i's values are residuals
- *     against the motion-compensated frame base_frame+i (what a gather with motion_values 1 returns), added per sample to
- *     pred(y, x) = frame(clamp(y + dy), clamp(x + dx)) at the selected pixels; the other pixels are copied.  fields holds
- *     count x mv_blocks x 2 int8 (dx, dy per 16 x 16 block, raster order; what rbf_stream_motion_search returns), one field per
- *     pair, read for mode 2 pairs only; it may be NULL when no pair has mode 2.  A mode above 2 or a vector component outside
- *     [-16, 16] is RBF_ERR_INVALID before anything is launched.  The modes and fields travel in the same H2D copy as the offsets.
- *     Runs of mode 0 / 1 pairs are applied by one K4c sweep each, every mode 2 pair by its own kernel, behind one tile count and
- *     scan for the whole chain on one CUDA stream; ivc:882, the first-bad-pair rule and slot wrap-around hold as above.
+ *     base_frame+i with mask slot i applied, i < count, using the value bytes [value_offsets[i], value_offsets[i+1]) of
+ *     `values` (host), or, when values is NULL, of the bytes the last rbf_stream_inflate_values placed on the device.  Pair i's
+ *     value mode is modes[i] (modes NULL: every pair 0):
+ *       0  the set pixels are replaced, in rank order, by the values;
+ *       1  the values are residuals (what a gather with value_mode 1 returns), added to the set pixels per sample
+ *          mod 2^(8 sample_bytes);
+ *       2  the values are residuals against the motion-compensated frame base_frame+i (what a gather with motion_values 1
+ *          returns), added per sample to pred(y, x) = frame(clamp(y + dy), clamp(x + dx)) at the set pixels; the other pixels
+ *          are copied.  fields holds count x mv_blocks x 2 int8 (dx, dy per 16 x 16 block, raster order; what
+ *          rbf_stream_motion_search returns), one field per pair, read for mode 2 pairs only; it may be NULL when no pair has
+ *          mode 2 and is not read when modes is NULL.
+ *     Refused with RBF_ERR_INVALID before anything is launched: decreasing offsets, a mode above 2, a mode 2 pair without
+ *     fields, a vector component outside [-16, 16], a chain that does not fit the store, and, when values is NULL, more value
+ *     bytes than were placed.  A call with values NULL ends the use of the placed bytes, whatever its outcome past that check.
+ *     One H2D copy of the host values, and one of the offsets (with the modes and the fields behind them when modes is given);
+ *     one synchronisation.  Runs of mode 0 / 1 pairs are applied by one K4c sweep each, every mode 2 pair by its own kernel,
+ *     behind one tile count and scan for the whole chain on one CUDA stream.  Frame slots are taken modulo max_frames, so a
+ *     chain may continue from the last frame of the previous one wherever it sits; count < max_frames.  ivc:882 per pair: pair
+ *     i is applied only if its mask's popcount x pixel bytes equals its value bytes; the first pair that fails gets
+ *     applied_out[i] = 0 and no frame from there on is written.  applied_out[i] = pixels applied.
  * rbf_stream_download_batch  frames first .. first+count-1 (slots modulo max_frames) into one contiguous host array, one
  *     synchronisation. */
 int rbf_stream_decode_masks(rbf_stream* s, uint32_t count, const uint8_t* bitmaps_packbits, uint64_t bitmap_slot_bytes,
                             const uint8_t* witness_packbits, uint64_t witness_slot_bytes, const uint64_t* l, const uint64_t* wlen,
                             const double* k, const uint8_t* raw, const rbf_seeds* seeds, uint64_t* consumed_out, uint64_t* ones_out);
-int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values, const uint64_t* value_offsets,
-                           uint64_t* applied_out);
-int rbf_stream_apply_chain_modes(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
-                                 const uint64_t* value_offsets, const uint8_t* residual /* [count] or NULL */, uint64_t* applied_out);
-int rbf_stream_apply_chain_motion(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
-                                  const uint64_t* value_offsets, const uint8_t* modes /* [count] */,
-                                  const int8_t* fields /* [count][mv_blocks][2] or NULL */, uint64_t* applied_out);
+int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values /* or NULL: on the device */,
+                           const uint64_t* value_offsets /* [count + 1] */, const uint8_t* modes /* [count] or NULL */,
+                           const int8_t* fields /* [count][mv_blocks][2] or NULL */, uint64_t* applied_out);
 /* Block motion search of pairs [0, pairs) of the last encode, prev -> curr: 16 x 16 blocks in raster order (mv_blocks =
  * ceil(H/16) x ceil(W/16), edge blocks clipped to the frame); per block the (dx, dy) in [-16, 16]^2 that minimises the SAD over the
  * block's pixels and samples of |curr - pred|, pred(y, x) = prev(clamp(y + dy, 0, H-1), clamp(x + dx, 0, W-1)); ties go to the
@@ -290,13 +288,11 @@ int rbf_inflate_segment(const uint8_t* in, uint64_t avail, uint8_t* out, uint32_
 int rbf_zlib_decompress_batch(rbf_ctx* ctx, uint32_t count, const void* const* srcs, const uint64_t* lens, const uint64_t* bounds,
                               uint8_t* out_host, uint64_t out_capacity, uint64_t* out_offsets /* count+1 */, uint8_t* on_device);
 /* the value streams of a decoded group (bounds[i]: pair i's value bytes, vcount x sample bytes): inflated into a device buffer of
- * the stream, the accepted ones back to back, out_lens[i] bytes each (0 when declined).  rbf_stream_apply_chain_inflated then
- * runs rbf_stream_apply_chain_motion on them (value_offsets[count] must not exceed what was placed; fields may be NULL when no
- * mode is 2), so the inflated values never cross PCIe.  The next inflate_values, or the apply, ends their use. */
+ * the stream, the accepted ones back to back, out_lens[i] bytes each (0 when declined).  rbf_stream_apply_chain with values NULL
+ * then reconstructs from them (value_offsets[count] must not exceed what was placed), so the inflated values never cross PCIe.
+ * The next inflate_values, or that apply, ends their use. */
 int rbf_stream_inflate_values(rbf_stream* s, uint32_t count, const void* const* srcs, const uint64_t* lens, const uint64_t* bounds,
                               uint64_t* out_lens, uint8_t* on_device);
-int rbf_stream_apply_chain_inflated(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint64_t* value_offsets,
-                                    const uint8_t* modes, const int8_t* fields, uint64_t* applied_out);
 
 /* ------------------------------------------------------------------ multi-GPU (one process per GPU)
  * frames are sharded across ranks; the per-rank Bloom bit arrays are exchanged with ONE ncclAllGather

@@ -32,7 +32,7 @@ class MaskInfo(C.Structure):
                 ("floor_k", C.c_uint32), ("raw", C.c_uint32)]
 
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 IVC_SEEDS = (0x12345678, 0x87654321, 999)    # improved_video_compressor.py:62-63,94
 BC_SEEDS = (0, 1, 999)                       # bloom_compress.py:163-164,195
 
@@ -49,10 +49,9 @@ EXPORTS = [
     "rbf_stream_create", "rbf_stream_destroy", "rbf_stream_set_option", "rbf_stream_upload", "rbf_stream_frame_ptr", "rbf_stream_encode",
     "rbf_stream_encode_host", "rbf_stream_fetch", "rbf_stream_fetch_batch", "rbf_stream_decode_verify", "rbf_stream_bitmap_region", "rbf_stream_stage_ms",
     "rbf_stream_gather_changed", "rbf_stream_apply_diff", "rbf_stream_download", "rbf_median_blur5", "rbf_stream_median5",
-    "rbf_stream_decode_masks", "rbf_stream_apply_chain", "rbf_stream_apply_chain_modes", "rbf_stream_apply_chain_motion",
-    "rbf_stream_motion_search", "rbf_stream_download_batch",
+    "rbf_stream_decode_masks", "rbf_stream_apply_chain", "rbf_stream_motion_search", "rbf_stream_download_batch",
     "rbf_zlib_bound", "rbf_deflate_code_lengths", "rbf_zlib_compress_batch", "rbf_stream_zlib_changed",
-    "rbf_inflate_segment", "rbf_zlib_decompress_batch", "rbf_stream_inflate_values", "rbf_stream_apply_chain_inflated",
+    "rbf_inflate_segment", "rbf_zlib_decompress_batch", "rbf_stream_inflate_values",
     "rbf_nccl_unique_id", "rbf_nccl_init", "rbf_nccl_allgather", "rbf_stream_allgather_bitmaps", "rbf_nccl_destroy",
     "rbf_peer_export", "rbf_peer_open", "rbf_peer_close", "rbf_peer_gather_init", "rbf_peer_gather_half", "rbf_peer_gather_shutdown",
 ]
@@ -122,9 +121,7 @@ def _sig(L):
     L.rbf_stream_apply_diff.argtypes = [vp, u32, u32, vp, vp, u64, P(u64)]
     L.rbf_stream_download.argtypes = [vp, u32, vp]
     L.rbf_stream_decode_masks.argtypes = [vp, u32, vp, u64, vp, u64, vp, vp, vp, vp, P(Seeds), vp, vp]
-    L.rbf_stream_apply_chain.argtypes = [vp, u32, u32, vp, vp, vp]
-    L.rbf_stream_apply_chain_modes.argtypes = [vp, u32, u32, vp, vp, vp, vp]
-    L.rbf_stream_apply_chain_motion.argtypes = [vp, u32, u32, vp, vp, vp, vp, vp]
+    L.rbf_stream_apply_chain.argtypes = [vp, u32, u32, vp, vp, vp, vp, vp]
     L.rbf_stream_motion_search.argtypes = [vp, u32, vp]
     L.rbf_stream_download_batch.argtypes = [vp, u32, u32, vp]
     L.rbf_median_blur5.argtypes = [vp, vp, u32, u32, u32, vp]
@@ -137,7 +134,6 @@ def _sig(L):
     L.rbf_inflate_segment.argtypes = [vp, u64, vp, P(u32), P(u64), P(u32), P(u32), P(u32)]
     L.rbf_zlib_decompress_batch.argtypes = [vp, u32, vp, vp, vp, vp, u64, vp, vp]
     L.rbf_stream_inflate_values.argtypes = [vp, u32, vp, vp, vp, vp, vp]
-    L.rbf_stream_apply_chain_inflated.argtypes = [vp, u32, u32, vp, vp, vp, vp]
     L.rbf_nccl_unique_id.argtypes = [vp]
     L.rbf_nccl_init.argtypes = [vp, vp, i32, i32]
     L.rbf_nccl_allgather.argtypes = [vp, vp, vp, u64]

@@ -616,9 +616,9 @@ struct rbf_stream {
     int motion_values = 0;  // 1: the gathers return residuals against the motion-compensated previous frame of the last search
     int8_t* d_fields = nullptr;             // [max_pairs][mv_blocks(H, W)][2] block vectors of rbf_stream_motion_search
     uint32_t motion_pairs = 0;              // pairs searched since the last encode (0: none, or a decode_masks overwrote the slots)
-    uint8_t* d_inflated = nullptr;          // rbf_stream_inflate_values: the group's values back to back, read by apply_chain_inflated
+    uint8_t* d_inflated = nullptr;          // rbf_stream_inflate_values: the group's values back to back, read by apply_chain (values NULL)
     size_t inflated_cap = 0;
-    uint64_t inflated_bytes = 0;            // bytes the last rbf_stream_inflate_values placed (cleared by apply_chain_inflated)
+    uint64_t inflated_bytes = 0;            // bytes the last rbf_stream_inflate_values placed (cleared by apply_chain with values NULL)
     bool last_k1_only = false;
     rbf_seeds last_sd = {};                 // seeds of the last encode (decode_verify rebuilds its jobs from them and last_infos)
     size_t bits_hwm = 0, wit_hwm = 0;   // bytes per slot that may hold set bits (see enc_stage_jobs)
@@ -1350,17 +1350,16 @@ extern "C" int rbf_stream_decode_masks(rbf_stream* s, uint32_t count, const uint
 }
 
 extern "C" int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
-                                      const uint64_t* value_offsets, uint64_t* applied_out) {
-    return rbf_stream_apply_chain_modes(s, base_frame, count, values, value_offsets, nullptr, applied_out);
-}
-
-// rbf_stream_apply_chain_modes / _motion: modes[i] <= max_mode (NULL: every pair plain); fields [count][nblocks][2] for mode 2 pairs
-// d_values (device): the values are already there, as rbf_stream_inflate_values leaves them, and `values` is not read
-static int apply_chain_impl(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values, const uint64_t* value_offsets,
-                            const uint8_t* modes, uint8_t max_mode, const int8_t* fields, uint64_t* applied_out,
-                            const uint8_t* d_values = nullptr) {
+                                      const uint64_t* value_offsets, const uint8_t* modes, const int8_t* fields, uint64_t* applied_out) {
     if (!s || !value_offsets || !applied_out) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_apply_chain: NULL");
     rbf_ctx* c = s->c;
+    const uint64_t vbytes = value_offsets[count];
+    if (!values) {                                       // the bytes the last rbf_stream_inflate_values placed, read by one call
+        if (vbytes > s->inflated_bytes)
+            return set_err(c, RBF_ERR_INVALID, "rbf_stream_apply_chain: %llu value bytes, %llu inflated", (unsigned long long)vbytes,
+                           (unsigned long long)s->inflated_bytes);
+        s->inflated_bytes = 0;
+    }
     if (count == 0 || count > s->max_pairs || count >= s->max_frames || base_frame >= s->max_frames)
         return set_err(c, RBF_ERR_INVALID, "chain of %u frames from slot %u does not fit a store of %u frames / %u pairs", count,
                        base_frame, s->max_frames, s->max_pairs);
@@ -1368,35 +1367,31 @@ static int apply_chain_impl(rbf_stream* s, uint32_t base_frame, uint32_t count, 
         if (value_offsets[i + 1] < value_offsets[i]) return set_err(c, RBF_ERR_INVALID, "value offsets decrease at pair %u", i);
     bool any_residual = false, any_motion = false;
     for (uint32_t i = 0; modes && i < count; i++) {
-        if (modes[i] > max_mode)
-            return set_err(c, RBF_ERR_INVALID, max_mode == 1 ? "pair %u: residual flag %u is neither 0 nor 1" : "pair %u: value mode %u is not 0, 1 or 2",
-                           i, (unsigned)modes[i]);
+        if (modes[i] > 2) return set_err(c, RBF_ERR_INVALID, "pair %u: value mode %u is not 0, 1 or 2", i, (unsigned)modes[i]);
         any_residual |= modes[i] == 1;
         any_motion |= modes[i] == 2;
     }
-    const size_t field_bytes = fields ? (size_t)count * mv_blocks(s->H, s->W) * 2 : 0;
-    if (any_motion && !fields) return set_err(c, RBF_ERR_INVALID, "rbf_stream_apply_chain_motion: motion pairs without fields");
+    const size_t field_bytes = modes && fields ? (size_t)count * mv_blocks(s->H, s->W) * 2 : 0;
+    if (any_motion && !fields) return set_err(c, RBF_ERR_INVALID, "rbf_stream_apply_chain: motion pairs without fields");
     for (size_t i = 0; i < field_bytes; i++)
         if (fields[i] < -MV_RANGE || fields[i] > MV_RANGE)
             return set_err(c, RBF_ERR_INVALID, "pair %llu: motion vector component %d is outside [-%d, %d]",
                            (unsigned long long)(i / (field_bytes / count)), (int)fields[i], MV_RANGE, MV_RANGE);
-    const uint64_t vbytes = value_offsets[count];
-    if (vbytes && !values && !d_values) return set_err(c, RBF_ERR_INVALID, "rbf_stream_apply_chain: values is NULL");
     CK(c, cudaSetDevice(c->device));
     const uint32_t ntiles = (uint32_t)((s->npix + AP_TILE_PX - 1) / AP_TILE_PX);
-    void *d_vals, *d_small, *d_pfx;
+    const bool on_device = !values && vbytes;            // the values are where rbf_stream_inflate_values left them
+    void *d_vals = s->d_inflated, *d_small, *d_pfx;
     int rc;
     // d_small: the value offsets, then the modes, then the fields (one H2D copy for all three), then first_bad and the totals
     const size_t off_bytes = 8 * ((size_t)count + 1), flag_bytes = modes ? count : 0;
     const size_t res_at = align_up(off_bytes + flag_bytes + field_bytes, 16);
     const size_t small = res_at + 4 * ((size_t)count + 1) + (field_bytes ? 4 * (size_t)count : 0);   // + the runs' first_bad words
-    d_vals = (void*)d_values;
-    if ((!d_values && (rc = scratch_get(c, kScrValues, (size_t)vbytes + 256, &d_vals))) || (rc = scratch_get(c, kScrChainSmall, small, &d_small)) ||
+    if ((!on_device && (rc = scratch_get(c, kScrValues, (size_t)vbytes + 256, &d_vals))) || (rc = scratch_get(c, kScrChainSmall, small, &d_small)) ||
         (rc = scratch_get(c, kScrChainTiles, 4 * (size_t)count * ntiles, &d_pfx)))
         return rc;
     uint64_t* d_off = (uint64_t*)d_small;
     uint32_t* d_res = (uint32_t*)((uint8_t*)d_small + res_at);   // [0] first_bad, [1 + i] totals
-    if (vbytes && !d_values) { CK(c, cudaMemcpyAsync(d_vals, values, (size_t)vbytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)vbytes; }
+    if (values && vbytes) { CK(c, cudaMemcpyAsync(d_vals, values, (size_t)vbytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)vbytes; }
     if (modes) {
         std::vector<uint8_t> head(off_bytes + flag_bytes + field_bytes);
         memcpy(head.data(), value_offsets, off_bytes);
@@ -1416,32 +1411,15 @@ static int apply_chain_impl(rbf_stream* s, uint32_t base_frame, uint32_t count, 
     A.values = (const uint8_t*)d_vals; A.value_off = d_off;
     A.sample_bytes = s->S;
     A.tile_pfx = (uint32_t*)d_pfx; A.totals = d_res + 1; A.first_bad = d_res;
-    if (any_motion) {                                    // split at the motion pairs
-        A.residual = (const uint8_t*)d_small + off_bytes;
-        CK(c, launch_apply_chain_motion(c->L, A, modes, (const int8_t*)d_small + off_bytes + flag_bytes, s->H, s->W,
-                                        d_res + 1 + count, c->st));
-    } else {
-        A.residual = any_residual ? (const uint8_t*)d_small + off_bytes : nullptr;   // a group without residual pairs runs the plain sweep
-        CK(c, launch_apply_chain(c->L, A, c->st));
-    }
+    A.residual = any_residual || any_motion ? (const uint8_t*)d_small + off_bytes : nullptr;
+    CK(c, launch_apply_chain(c->L, A, modes, field_bytes ? (const int8_t*)d_small + off_bytes + flag_bytes : nullptr, s->H, s->W,
+                             d_res + 1 + count, c->st));
     std::vector<uint32_t> h((size_t)count + 1);
     CK(c, cudaMemcpyAsync(h.data(), d_res, 4 * ((size_t)count + 1), cudaMemcpyDeviceToHost, c->st));
     c->d2h += 4 * ((int64_t)count + 1);
     CK(c, cudaStreamSynchronize(c->st));
     for (uint32_t i = 0; i < count; i++) applied_out[i] = i < h[0] ? h[1 + i] : 0;
     return RBF_OK;
-}
-
-extern "C" int rbf_stream_apply_chain_modes(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
-                                            const uint64_t* value_offsets, const uint8_t* residual, uint64_t* applied_out) {
-    return apply_chain_impl(s, base_frame, count, values, value_offsets, residual, 1, nullptr, applied_out);
-}
-
-extern "C" int rbf_stream_apply_chain_motion(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
-                                             const uint64_t* value_offsets, const uint8_t* modes, const int8_t* fields,
-                                             uint64_t* applied_out) {
-    if (!modes) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_apply_chain_motion: modes is NULL");
-    return apply_chain_impl(s, base_frame, count, values, value_offsets, modes, 2, fields, applied_out);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1843,17 +1821,6 @@ extern "C" int rbf_stream_inflate_values(rbf_stream* s, uint32_t count, const vo
     if (int rc = inflate_place(c, R, off.data(), s->d_inflated, total)) return rc;
     s->inflated_bytes = total;
     return RBF_OK;
-}
-
-extern "C" int rbf_stream_apply_chain_inflated(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint64_t* value_offsets,
-                                               const uint8_t* modes, const int8_t* fields, uint64_t* applied_out) {
-    if (!s || !value_offsets || !modes) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_apply_chain_inflated: NULL");
-    if (count && value_offsets[count] > s->inflated_bytes)
-        return set_err(s->c, RBF_ERR_INVALID, "rbf_stream_apply_chain_inflated: %llu value bytes, %llu inflated",
-                       (unsigned long long)value_offsets[count], (unsigned long long)s->inflated_bytes);
-    const int rc = apply_chain_impl(s, base_frame, count, nullptr, value_offsets, modes, 2, fields, applied_out, s->d_inflated);
-    s->inflated_bytes = 0;
-    return rc;
 }
 
 // ------------------------------------------------------------------------------------------

@@ -469,22 +469,20 @@ static void launch_tile_prefix(LaunchCfg& L, const ApplyChain& A, cudaStream_t s
     k_tile_scan<<<A.count, 1024, 0, st>>>(A);
     L.launches += 2;
 }
-cudaError_t launch_apply_chain(LaunchCfg& L, const ApplyChain& A, cudaStream_t st) {
+cudaError_t launch_apply_chain(LaunchCfg& L, const ApplyChain& A, const uint8_t* h_modes, const int8_t* d_fields, uint32_t H,
+                               uint32_t W, uint32_t* d_run_bad, cudaStream_t st) {
     if (A.count == 0 || A.ntiles == 0) return cudaSuccess;
-    const uint32_t key = A.pix_bytes * 4u + (A.residual ? A.sample_bytes : 0u);
-    if (!apply_key_ok(key)) return cudaErrorInvalidValue;
-    launch_tile_prefix(L, A, st);
-    return launch_sweep(L, A, key, st);
-}
-cudaError_t launch_apply_chain_motion(LaunchCfg& L, const ApplyChain& A, const uint8_t* h_modes, const int8_t* d_fields, uint32_t H,
-                                     uint32_t W, uint32_t* d_run_bad, cudaStream_t st) {
-    if (A.count == 0 || A.ntiles == 0) return cudaSuccess;
+    auto mode = [&](uint32_t t) -> uint8_t { return h_modes ? h_modes[t] : 0; };
+    bool any_residual = false, any_motion = false;
+    for (uint32_t t = 0; t < A.count; t++) { any_residual |= mode(t) == 1; any_motion |= mode(t) == 2; }
     const uint32_t mkey = A.pix_bytes * 4u + A.sample_bytes;           // the residual kinds of launch_gather_scatter
-    if (!A.residual || !d_fields || !apply_key_ok(mkey) || mkey == A.pix_bytes * 4u) return cudaErrorInvalidValue;
+    if (!apply_key_ok(A.pix_bytes * 4u + (any_residual ? A.sample_bytes : 0u)) || ((any_residual || any_motion) && !A.residual) ||
+        (any_motion && (!d_fields || !apply_key_ok(mkey) || mkey == A.pix_bytes * 4u)))
+        return cudaErrorInvalidValue;
     launch_tile_prefix(L, A, st);
     for (uint32_t t = 0; t < A.count;) {
-        if (h_modes[t] == 2) {
-            uint32_t* next_bad = t + 1u < A.count && h_modes[t + 1u] != 2 ? d_run_bad + t + 1u : nullptr;
+        if (mode(t) == 2) {
+            uint32_t* next_bad = t + 1u < A.count && mode(t + 1u) != 2 ? d_run_bad + t + 1u : nullptr;
             switch (mkey) {
             case 1u * 4 + 1: k_apply_motion<1, 1><<<A.ntiles, AP_THREADS, 0, st>>>(A, t, d_fields, H, W, next_bad); break;
             case 3u * 4 + 1: k_apply_motion<3, 1><<<A.ntiles, AP_THREADS, 0, st>>>(A, t, d_fields, H, W, next_bad); break;
@@ -495,20 +493,20 @@ cudaError_t launch_apply_chain_motion(LaunchCfg& L, const ApplyChain& A, const u
             t++;
             continue;
         }
-        // a run of plain / residual pairs [t, t1) is swept as a chain of its own; a run after a motion pair checks the first failing
-        // pair counted from its start, which that motion kernel stored
+        // a run of plain / residual pairs [t, t1) is swept as a chain of its own (without a motion pair: the whole chain, A as
+        // given); a run after a motion pair checks the first failing pair counted from its start, which that motion kernel stored
         uint32_t t1 = t;
-        bool any_residual = false;
-        for (; t1 < A.count && h_modes[t1] != 2; t1++) any_residual |= h_modes[t1] != 0;
+        bool run_residual = false;
+        for (; t1 < A.count && mode(t1) != 2; t1++) run_residual |= mode(t1) != 0;
         ApplyChain R = A;
         R.masks = A.masks + (size_t)t * A.mask_stride_w;
         R.base = A.base + t >= A.max_frames ? A.base + t - A.max_frames : A.base + t;
         R.count = t1 - t;
         R.value_off = A.value_off + t;
-        R.residual = any_residual ? A.residual + t : nullptr;
+        R.residual = run_residual ? A.residual + t : nullptr;
         R.tile_pfx = A.tile_pfx + (size_t)t * A.ntiles;
         R.first_bad = t == 0 ? A.first_bad : d_run_bad + t;
-        if (cudaError_t e = launch_sweep(L, R, A.pix_bytes * 4u + (any_residual ? A.sample_bytes : 0u), st)) return e;
+        if (cudaError_t e = launch_sweep(L, R, A.pix_bytes * 4u + (run_residual ? A.sample_bytes : 0u), st)) return e;
         t = t1;
     }
     return cudaSuccess;

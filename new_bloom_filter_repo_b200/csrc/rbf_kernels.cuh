@@ -164,14 +164,14 @@ cudaError_t launch_raw_masks(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32
 cudaError_t launch_mask_popcount(LaunchCfg& L, const uint32_t* d_masks, size_t stride_w, uint32_t npix, int F, uint32_t* d_out,
                                  cudaStream_t st);
 // K4c: tile counts, tile scan (+ the ivc:882 check) and the chained sweep; *A.first_bad must hold UINT32_MAX before the launch.
-// A.residual == NULL runs the plain sweep, which has no residual branch at all
-cudaError_t launch_apply_chain(LaunchCfg& L, const ApplyChain& A, cudaStream_t st);
-// K4c with motion pairs: h_modes[t] (host) is 0 plain, 1 residual, 2 motion-compensated residual; A.residual holds the same modes on
-// the device, d_fields the [count][mv_blocks(H, W)][2] block vectors.  One tile count + scan for the whole chain, then one
-// k_apply_sweep per run of plain / residual pairs and one k_apply_motion per motion pair, in order on `st`.  d_run_bad: count words
-// of scratch (a run's first failing pair, counted from the run's start).
-cudaError_t launch_apply_chain_motion(LaunchCfg& L, const ApplyChain& A, const uint8_t* h_modes, const int8_t* d_fields, uint32_t H,
-                                     uint32_t W, uint32_t* d_run_bad, cudaStream_t st);
+// h_modes[t] (host; NULL: every pair 0) is 0 plain, 1 residual, 2 motion-compensated residual; A.residual holds the same modes on
+// the device (needed when a mode is not 0), d_fields the [count][mv_blocks(H, W)][2] block vectors (needed when a mode is 2).  One
+// tile count + scan for the whole chain, then one k_apply_sweep per run of plain / residual pairs and one k_apply_motion per motion
+// pair, in order on `st`; a run without a residual pair gets the plain sweep, which has no residual branch at all.  Without a motion
+// pair the one run is the whole chain and gets A's arguments.  d_run_bad: count words of scratch (a run's first failing pair, counted
+// from the run's start), read only after a motion pair.
+cudaError_t launch_apply_chain(LaunchCfg& L, const ApplyChain& A, const uint8_t* h_modes, const int8_t* d_fields, uint32_t H,
+                               uint32_t W, uint32_t* d_run_bad, cudaStream_t st);
 cudaError_t launch_median5(LaunchCfg& L, const void* d_in, uint32_t pix_stride, uint32_t H, uint32_t W, int sample_bytes, void* d_out,
                            cudaStream_t st);
 cudaError_t launch_bitrev(LaunchCfg& L, uint32_t* d_words, size_t nwords, cudaStream_t st);

@@ -761,11 +761,10 @@ class ImprovedVideoCompressor:
             if ones[i] != j.p.ones:                          # the reference would silently return the base frame (ivc:882)
                 raise ValueError(f"corrupt inter frame: the decoded mask selects {int(ones[i])} pixels, the payload announces {j.p.ones}")
         if group[0].vlen is not None:                        # the group's values are on the device (_inflate_group)
-            applied = st.apply_chain_inflated(base, [j.vsize * j.p.isz for j in group], [j.p.vmode for j in group],
-                                              motion=[j.field_arr for j in group])
+            vals = {"inflated": [j.vsize * j.p.isz for j in group]}
         else:
-            applied = st.apply_chain(base, [j.values_arr for j in group], residual=[j.p.vmode for j in group],
-                                     motion=[j.field_arr for j in group])
+            vals = {"values": [j.values_arr for j in group]}
+        applied = st.apply_chain(base, **vals, modes=[j.p.vmode for j in group], motion=[j.field_arr for j in group])
         if not np.array_equal(applied, ones):
             raise ValueError(f"corrupt inter frame: {applied.tolist()} pixels applied, {ones.tolist()} expected")
         return st.download_batch((base + 1) % st.max_frames, m)

@@ -222,35 +222,42 @@ class FrameStream:
         self.pairs = 0
         return consumed, ones
 
-    def apply_chain(self, base_frame: int, values: Sequence[np.ndarray], residual: Optional[Sequence[int]] = None,
-                    motion: Optional[Sequence[Optional[np.ndarray]]] = None) -> np.ndarray:
-        """Frame base_frame+1+i = frame base_frame+i with mask slot i applied, values[i] replacing its set pixels in rank order
-        (ivc:849-909), for i < len(values); slots are taken modulo max_frames.  residual[i] = 1 adds values[i] to the set pixels
-        per sample (mod 2^bits) instead: the residuals a value_mode=1 gather returns.  residual[i] = 2 adds them to the motion-compensated
-        prediction from frame base_frame+i under motion[i], pair i's int8 field of motion_search's shape [by, bx, 2] (motion[j] is
-        ignored, and may be None, for the other pairs): the residuals a motion_values=1 gather returns.  A mode-2 pair whose motion[i]
-        is None raises ValueError; without `motion` the flags go to rbf_stream_apply_chain_modes, which refuses 2.  -> uint64[count] pixels applied
-        per pair: 0 from the first pair whose value count does not match its mask (ivc:882), whose frame and every later one are not
-        written."""
-        parts = [memoryview(np.ascontiguousarray(v)).cast("B") for v in values]
-        offs = np.zeros(len(parts) + 1, dtype=np.uint64)
-        offs[1:] = np.cumsum([p.nbytes for p in parts])
-        buf = np.frombuffer(b"".join(parts), dtype=np.uint8)
-        applied = np.zeros(len(parts), dtype=np.uint64)
-        flags = None
-        if residual is not None:
-            flags = np.ascontiguousarray(np.asarray(residual, dtype=np.uint8))
-            if flags.shape != (len(parts),):
-                raise ValueError("one residual flag per pair")
-        if motion is not None and flags is not None and (flags == 2).any():
-            fields = self._motion_fields(flags, motion)
-            _cabi.check(_cabi.lib().rbf_stream_apply_chain_motion(self._h, int(base_frame), len(parts), _cabi.ptr(buf) if buf.size else None,
-                                                                  _cabi.ptr(offs), _cabi.ptr(flags), _cabi.ptr(fields), _cabi.ptr(applied)),
-                        _cabi.ctx())
-            return applied
-        _cabi.check(_cabi.lib().rbf_stream_apply_chain_modes(self._h, int(base_frame), len(parts), _cabi.ptr(buf) if buf.size else None,
-                                                             _cabi.ptr(offs), _cabi.ptr(flags) if flags is not None else None,
-                                                             _cabi.ptr(applied)), _cabi.ctx())
+    def apply_chain(self, base_frame: int, values: Optional[Sequence[np.ndarray]] = None, *, inflated: Optional[Sequence[int]] = None,
+                    modes: Optional[Sequence[int]] = None, motion: Optional[Sequence[Optional[np.ndarray]]] = None) -> np.ndarray:
+        """Frame base_frame+1+i = frame base_frame+i with mask slot i applied, pair i's values replacing its set pixels in rank order
+        (ivc:849-909), for every pair i; slots are taken modulo max_frames.  Pair i's values are either values[i] (host arrays) or,
+        with `inflated`, the first inflated[i] bytes of the i-th stream the last inflate_values placed (every one of them inflated
+        on the device, in order): those never cross PCIe, and the call ends their use.  Exactly one of the two is given.
+        modes[i] = 1 adds the values to the set pixels per sample (mod 2^bits) instead: the residuals a value_mode=1 gather returns.
+        modes[i] = 2 adds them to the motion-compensated prediction from frame base_frame+i under motion[i], pair i's int8 field
+        of motion_search's shape [by, bx, 2] (motion[j] is ignored, and may be None, for the other pairs): the residuals a
+        motion_values=1 gather returns.  A mode-2 pair whose motion[i] is None raises ValueError, and one without `motion` raises
+        RbfError.  -> uint64[count] pixels applied per pair: 0 from the first pair whose value count does not match its mask
+        (ivc:882), whose frame and every later one are not written."""
+        if (values is None) == (inflated is None):
+            raise ValueError("pass either values or inflated")
+        buf = None
+        if values is not None:
+            parts = [memoryview(np.ascontiguousarray(v)).cast("B") for v in values]
+            sizes = [p.nbytes for p in parts]
+            buf = np.frombuffer(b"".join(parts), dtype=np.uint8)
+        else:
+            sizes = np.asarray(inflated, dtype=np.uint64)
+        count = len(sizes)
+        offs = np.zeros(count + 1, dtype=np.uint64)
+        offs[1:] = np.cumsum(sizes)
+        applied = np.zeros(count, dtype=np.uint64)
+        flags = fields = None
+        if modes is not None:
+            flags = np.ascontiguousarray(np.asarray(modes, dtype=np.uint8))
+            if flags.shape != (count,):
+                raise ValueError("one value mode per pair")
+            if motion is not None and (flags == 2).any():
+                fields = self._motion_fields(flags, motion)
+        _cabi.check(_cabi.lib().rbf_stream_apply_chain(self._h, int(base_frame), count, _cabi.ptr(buf) if buf is not None and buf.size else None,
+                                                       _cabi.ptr(offs), _cabi.ptr(flags) if flags is not None else None,
+                                                       _cabi.ptr(fields) if fields is not None else None, _cabi.ptr(applied)),
+                    _cabi.ctx())
         return applied
 
     def _motion_fields(self, flags: np.ndarray, motion) -> np.ndarray:
@@ -267,7 +274,7 @@ class FrameStream:
         return fields
 
     def inflate_values(self, streams: Sequence, bounds: Sequence[int]):
-        """The zlib value streams of a group inflated on the GPU into the stream's value buffer, for apply_chain_inflated.
+        """The zlib value streams of a group inflated on the GPU into the stream's value buffer, for apply_chain(inflated=...).
         bounds[i]: the most stream i may hold (its value count x sample bytes).  -> (inflated bytes uint64[n], on_device bool[n]);
         a declined stream (not the device coder's layout, or larger than its bound) has on_device False and 0 bytes."""
         views = [np.frombuffer(memoryview(s).cast("B"), dtype=np.uint8) for s in streams]
@@ -280,22 +287,6 @@ class FrameStream:
         _cabi.check(_cabi.lib().rbf_stream_inflate_values(self._h, n, srcs, _cabi.ptr(lens), _cabi.ptr(bnd), _cabi.ptr(out), _cabi.ptr(ok)),
                     _cabi.ctx())
         return out, ok.astype(bool)
-
-    def apply_chain_inflated(self, base_frame: int, nbytes: Sequence[int], residual: Sequence[int],
-                             motion: Optional[Sequence[Optional[np.ndarray]]] = None) -> np.ndarray:
-        """apply_chain with pair i's values the first nbytes[i] bytes of the i-th stream the last inflate_values placed (every one
-        of them inflated on the device, in order): the values never cross PCIe."""
-        offs = np.zeros(len(nbytes) + 1, dtype=np.uint64)
-        offs[1:] = np.cumsum(np.asarray(nbytes, dtype=np.uint64))
-        flags = np.ascontiguousarray(np.asarray(residual, dtype=np.uint8))
-        if flags.shape != (len(nbytes),):
-            raise ValueError("one value mode per pair")
-        fields = self._motion_fields(flags, motion) if motion is not None and (flags == 2).any() else None
-        applied = np.zeros(len(nbytes), dtype=np.uint64)
-        _cabi.check(_cabi.lib().rbf_stream_apply_chain_inflated(self._h, int(base_frame), len(nbytes), _cabi.ptr(offs), _cabi.ptr(flags),
-                                                                _cabi.ptr(fields) if fields is not None else None, _cabi.ptr(applied)),
-                    _cabi.ctx())
-        return applied
 
     def download_batch(self, first: int, count: int) -> np.ndarray:
         """Frames first .. first+count-1 (slots modulo max_frames) -> [count, H, W(, C)], one copy and one synchronisation."""

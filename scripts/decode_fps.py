@@ -52,10 +52,10 @@ def per_frame_decode(comp, payloads):
 
 class StageTimer:
     """Device-event time (rbf_timer_start / rbf_timer_stop_ms on the context's stream) of FrameStream.decode_masks and
-    FrameStream.apply_chain -- or, for GPU-coded files, inflate_values and apply_chain_inflated -- per call."""
+    FrameStream.apply_chain -- and, for GPU-coded files, inflate_values -- per call."""
 
     def __init__(self):
-        self.ms = {"inflate_values": [], "decode_masks": [], "apply_chain": [], "apply_chain_inflated": []}
+        self.ms = {"inflate_values": [], "decode_masks": [], "apply_chain": []}
         self._orig = {}
 
     def __enter__(self):
@@ -117,8 +117,7 @@ def run(h, w, coder, runs=3):
             "identical_frames": True,
             "decode_masks_ms_per_group": [round(x, 3) for x in tm.ms["decode_masks"]],
             "apply_chain_ms_per_group": [round(x, 3) for x in tm.ms["apply_chain"]],
-            "inflate_values_ms_per_group": [round(x, 3) for x in tm.ms["inflate_values"]],
-            "apply_chain_inflated_ms_per_group": [round(x, 3) for x in tm.ms["apply_chain_inflated"]]}
+            "inflate_values_ms_per_group": [round(x, 3) for x in tm.ms["inflate_values"]]}
 
 
 if __name__ == "__main__":

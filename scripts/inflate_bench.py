@@ -6,7 +6,7 @@
 2. decompress_video frames/s of GPU-coded 1080p x 30 and 4K x 30 YUV444 GOPs: the device route and the host route (every value
    stream and keyframe blob inflated with zlib.decompress, forced here by substituting the host inflater), alternated, 3 runs
    each, identical frames required.
-3. Per group of the device route: device-event time of inflate_values, decode_masks and apply_chain_inflated, and host wall time.
+3. Per group of the device route: device-event time of inflate_values, decode_masks and apply_chain, and host wall time.
 The card's name and power limit are read in the same command.  One JSON line per result."""
 import ctypes
 import json
@@ -84,7 +84,7 @@ class HostRoute:
 
 class StageTimer:
     """Device-event time per call of the named FrameStream methods, and host wall time of each decompress_video group."""
-    NAMES = ("inflate_values", "decode_masks", "apply_chain_inflated")
+    NAMES = ("inflate_values", "decode_masks", "apply_chain")
 
     def __enter__(self):
         L, ctx = _cabi.lib(), _cabi.ctx()

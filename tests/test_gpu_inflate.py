@@ -114,6 +114,41 @@ def test_malformed_streams_match_zlib(pkg):
         _deflate().decompress(dict(_bad_streams())["bad-adler"])
 
 
+# ------------------------------------------------------------------ FrameStream.apply_chain(inflated=...)
+@gpu
+def test_apply_chain_reads_inflated_values_once(pkg):
+    """The values inflate_values placed serve one apply_chain(inflated=...): asking for more bytes than were placed raises and
+    leaves them in place, a valid call reconstructs the frames that values= gives with the same bytes, and a second call raises."""
+    from tests.test_gpu_motion import _raw_slots
+    h, w, ch, cnt = 48, 40, 3, 4
+    n = h * w
+    rng = np.random.default_rng(44)
+    masks = [(rng.random(n) < p).astype(np.uint8) for p in (0.3, 0.0, 1.0, 0.05)]
+    vals = [rng.integers(0, 256, int(m.sum()) * ch).astype(np.uint8) for m in masks]
+    nbytes = [v.nbytes for v in vals]
+    modes = [0, 1, 0, 1]
+    base = rng.integers(0, 256, (h, w, ch)).astype(np.uint8)
+    st = pkg.FrameStream(h, w, ch, np.uint8, max_frames=cnt + 1, max_pairs=cnt, k1_only=True)
+    try:
+        _, ones = st.decode_masks(_raw_slots(masks, n), np.zeros((cnt, 0), np.uint8), [0] * cnt, [0] * cnt, [0.0] * cnt, [1] * cnt)
+        lens, ok = st.inflate_values(_deflate().compress_many([v.tobytes() for v in vals]), nbytes)
+        assert ok.all() and list(lens) == nbytes
+        with pytest.raises(pkg.RbfError):
+            st.apply_chain(0, inflated=nbytes[:-1] + [nbytes[-1] + 1], modes=modes)
+        st.upload(base, first=0)
+        applied = st.apply_chain(0, inflated=nbytes, modes=modes)
+        got = st.download_batch(1, cnt)
+        with pytest.raises(pkg.RbfError):
+            st.apply_chain(0, inflated=nbytes, modes=modes)
+        st.upload(base, first=0)
+        assert list(applied) == list(st.apply_chain(0, vals, modes=modes)) == list(ones)
+        assert np.array_equal(got, st.download_batch(1, cnt))
+        with pytest.raises(ValueError):
+            st.apply_chain(0, vals, inflated=nbytes)
+    finally:
+        st.close()
+
+
 # ------------------------------------------------------------------ decompress_video
 def _frames(h, w, ch, dtype, nfr, seed, p_seq):
     f = synth_stream(h, w, nfr, seed, p_seq, dtype)

@@ -455,7 +455,7 @@ def test_apply_chain_motion_matches_model(pkg, h, w, ch, dtype):
         assert list(ones) == [int(m.sum()) for m in masks]
         exp = model(MODES, fields)
         st.upload(base, first=5)                           # the chain writes slots 6, 7, 0, 1, 2, 3
-        applied = st.apply_chain(5, vals, residual=MODES, motion=fields)
+        applied = st.apply_chain(5, vals, modes=MODES, motion=fields)
         assert list(applied) == list(ones)
         got = st.download_batch(6, cnt)
         for t in range(cnt):
@@ -466,7 +466,7 @@ def test_apply_chain_motion_matches_model(pkg, h, w, ch, dtype):
             short = [v[:-ch] if t == bad else v for t, v in enumerate(vals)]
             st.upload(base, first=0)
             st.upload(np.full((mf - 1,) + shape, 7, dtype=dtype), first=1)
-            applied = st.apply_chain(0, short, residual=MODES, motion=fields)
+            applied = st.apply_chain(0, short, modes=MODES, motion=fields)
             assert list(applied) == list(ones[:bad]) + [0] * (cnt - bad), bad
             got = st.download_batch(1, cnt)
             for t in range(cnt):
@@ -476,38 +476,46 @@ def test_apply_chain_motion_matches_model(pkg, h, w, ch, dtype):
                     assert (got[t] == 7).all(), (bad, t)
         # all motion, and no motion pair through the same entry point
         st.upload(base, first=0)
-        assert list(st.apply_chain(0, vals, residual=[2] * cnt, motion=[fields[2]] * cnt)) == list(ones)
+        assert list(st.apply_chain(0, vals, modes=[2] * cnt, motion=[fields[2]] * cnt)) == list(ones)
         exp_all = model([2] * cnt, [fields[2]] * cnt)
         got = st.download_batch(1, cnt)
         assert all(np.array_equal(got[t], exp_all[t]) for t in range(cnt))
         st.upload(base, first=0)
-        assert list(st.apply_chain(0, vals, residual=[0, 1, 0, 1, 0, 0], motion=fields)) == list(ones)   # fields unused: no motion pair
+        assert list(st.apply_chain(0, vals, modes=[0, 1, 0, 1, 0, 0], motion=fields)) == list(ones)   # fields unused: no motion pair
         exp_none = model([0, 1, 0, 1, 0, 0], fields)
         got = st.download_batch(1, cnt)
         assert all(np.array_equal(got[t], exp_none[t]) for t in range(cnt))
-        # errors, checked before any launch
+        # no modes: every pair plain, and fields passed anyway are not read
         L, ctx = pkg._cabi.lib(), pkg._cabi.ctx()
-        L.rbf_reset_counters(ctx)
-        with pytest.raises(ValueError):                    # a motion pair without a field
-            st.apply_chain(0, vals, residual=MODES, motion=fields[:3] + [None] + fields[4:])
-        with pytest.raises(RbfError):                      # without fields the flags go to apply_chain_modes, which refuses mode 2
-            st.apply_chain(0, vals, residual=MODES)
-        with pytest.raises(RbfError):
-            st.apply_chain(0, vals, residual=[0, 1, 3, 0, 0, 0], motion=fields)
         buf = np.concatenate([v.view(np.uint8) for v in vals])
         offs = np.concatenate([[0], np.cumsum([v.nbytes for v in vals])]).astype(np.uint64)
-        flags = np.array([0, 1, 2, 0, 0, 0], np.uint8)
         out = np.zeros(cnt, np.uint64)
         ptr = pkg._cabi.ptr
-        assert L.rbf_stream_apply_chain_modes(st._h, 0, cnt, ptr(buf), ptr(offs), ptr(flags), ptr(out)) == -1   # keeps rejecting 2
+        fl = np.full((cnt,) + nb, 100, np.int8)
+        st.upload(base, first=0)
+        assert L.rbf_stream_apply_chain(st._h, 0, cnt, ptr(buf), ptr(offs), None, ptr(fl), ptr(out)) == 0
+        assert list(out) == list(ones)
+        exp_plain = model([0] * cnt, fields)
+        got = st.download_batch(1, cnt)
+        assert all(np.array_equal(got[t], exp_plain[t]) for t in range(cnt))
+        # errors, checked before any launch
+        L.rbf_reset_counters(ctx)
+        with pytest.raises(ValueError):                    # a motion pair without a field
+            st.apply_chain(0, vals, modes=MODES, motion=fields[:3] + [None] + fields[4:])
+        with pytest.raises(RbfError):                      # without `motion` the motion pairs reach C without fields
+            st.apply_chain(0, vals, modes=MODES)
+        with pytest.raises(RbfError):
+            st.apply_chain(0, vals, modes=[0, 1, 3, 0, 0, 0], motion=fields)
         fl = np.zeros((cnt,) + nb, np.int8)
-        assert L.rbf_stream_apply_chain_motion(st._h, 0, cnt, ptr(buf), ptr(offs), ptr(flags), None, ptr(out)) == -1   # no fields
-        assert L.rbf_stream_apply_chain_motion(st._h, 0, cnt, ptr(buf), ptr(offs), None, ptr(fl), ptr(out)) == -1     # no modes
+        flags = np.array([0, 1, 2, 0, 0, 0], np.uint8)
+        assert L.rbf_stream_apply_chain(st._h, 0, cnt, ptr(buf), ptr(offs), ptr(flags), None, ptr(out)) == -1   # mode 2, no fields
+        flags[2] = 3
+        assert L.rbf_stream_apply_chain(st._h, 0, cnt, ptr(buf), ptr(offs), ptr(flags), ptr(fl), ptr(out)) == -1    # a mode of 3
         for v in (17, -17, -128):
             bad_f = [None if f is None else f.copy() for f in fields]
             bad_f[5][-1, -1, 1] = v
             with pytest.raises(RbfError):
-                st.apply_chain(0, vals, residual=MODES, motion=bad_f)
+                st.apply_chain(0, vals, modes=MODES, motion=bad_f)
         assert L.rbf_get_counter(ctx, b"kernel_launches") == 0 and L.rbf_get_counter(ctx, b"h2d_bytes") == 0
     finally:
         st.close()

@@ -1,7 +1,7 @@
 """Adaptive value coding of inter frames (value_coding="adaptive", 'RBF3' payloads): the value stream of each inter frame holds either
 the current samples at the changed pixels or their residuals (curr - prev) mod 2^bits per sample, whichever zlib stream is shorter.
 The device side -- the residual gather (value_mode 1 of rbf_stream_gather_changed / rbf_stream_zlib_changed) and the residual apply
-of K4c (rbf_stream_apply_chain_modes) -- is compared with the numpy forms below, and decompress_video with a frame-by-frame route
+of K4c (rbf_stream_apply_chain with value modes) -- is compared with the numpy forms below, and decompress_video with a frame-by-frame route
 built from the C oracle's mask decode and these numpy forms."""
 import hashlib
 import struct
@@ -263,7 +263,7 @@ def test_apply_chain_mixed_flags_matches_oracle(pkg, h, w, ch, dtype):
             exp.append(cur)
         # base in slot 3: the chain writes slots 4, 0, 1, 2 (slots wrap)
         st.upload(base, first=3)
-        applied = st.apply_chain(3, vals, residual=flags)
+        applied = st.apply_chain(3, vals, modes=flags)
         assert list(applied) == list(ones)
         got = st.download_batch(4, cnt)
         for t in range(cnt):
@@ -271,7 +271,7 @@ def test_apply_chain_mixed_flags_matches_oracle(pkg, h, w, ch, dtype):
         assert np.array_equal(st.download(3), base)
         # all pairs plain through the same entry point equals apply_chain without flags
         st.upload(base, first=0)
-        a0 = st.apply_chain(0, vals, residual=[0] * cnt)
+        a0 = st.apply_chain(0, vals, modes=[0] * cnt)
         g0 = st.download_batch(1, cnt)
         st.upload(base, first=0)
         a1 = st.apply_chain(0, vals)
@@ -286,15 +286,15 @@ def test_apply_chain_mixed_flags_matches_oracle(pkg, h, w, ch, dtype):
         st.upload(base, first=0)
         st.upload(sentinel, first=3)
         short = vals[:2] + [vals[2][:-ch]] + vals[3:]
-        applied = st.apply_chain(0, short, residual=mixed)
+        applied = st.apply_chain(0, short, modes=mixed)
         assert list(applied) == [ones[0], ones[1], 0, 0]
         got = st.download_batch(1, 4)
         assert np.array_equal(got[0], exp2[0]) and np.array_equal(got[1], exp2[1])
         assert (got[2] == 7).all() and (got[3] == 7).all()
         with pytest.raises(pkg._cabi.RbfError):
-            st.apply_chain(0, vals, residual=[0, 2, 0, 0])
+            st.apply_chain(0, vals, modes=[0, 2, 0, 0])
         with pytest.raises(ValueError):
-            st.apply_chain(0, vals, residual=[0, 1])
+            st.apply_chain(0, vals, modes=[0, 1])
     finally:
         st.close()
 
