@@ -7,6 +7,7 @@ device coder on the GPU and builds the frame with build_frame).
 """
 from __future__ import annotations
 
+import math
 import struct
 import zlib
 from typing import Dict, List
@@ -90,66 +91,53 @@ class FixedVideoCompressor:
     def compress_frame(self, frame) -> bytes:                                    # fvc:27-74
         return assemble_keyframe(frame, [zlib.compress(r, 9) for r in keyframe_raws(frame)])
 
-    def compress_frame_async(self, frame, pool):
-        """compress_frame with the (up to four) zlib level-9 blobs as separate jobs of `pool`; returns a callable that assembles
-        exactly the bytes compress_frame(frame) returns.  The keyframe of a GOP is the longest serial piece of compress_video."""
-        futs = [pool.submit(zlib.compress, r, 9) for r in keyframe_raws(frame)]
-        return lambda: assemble_keyframe(frame, [f.result() for f in futs])
-
     def decompress_frame(self, data: bytes):                                     # fvc:76-181
         return self.build_frame(data, zlib.decompress)
 
     @staticmethod
-    def keyframe_blobs(data: bytes):
-        """The layout parse of a keyframe payload: [(zlib blob, most bytes it may inflate to)] for the frame and, YUV frames,
-        the three planes, in payload order; the bounds are h w itemsize 4 for the frame and ph pw for a plane.  Raises
-        struct.error (or another exception) on a truncated layout, as decompress_frame would reach it."""
+    def _parts(data: bytes, inflate):
+        """The layout parse of a keyframe payload, one part at a time in payload order: ("frame", inflate(blob), (h, w, itemsize)),
+        then for a YUV payload ("format", its utf-8 bytes, None) and ("y_plane" | "u_plane" | "v_plane", inflate(blob), (ph, pw)).
+        Each blob is inflated as soon as its length is read, before the parse reads on, and each part is yielded before the next
+        is read, so errors arise in payload order.  Raises struct.error on a truncated layout."""
         h, w, isz = struct.unpack_from("<III", data, 0)
         (zlen,) = struct.unpack_from("<I", data, 12)
-        blobs = [(data[16:16 + zlen], h * w * isz * 4)]
+        yield "frame", inflate(data[16:16 + zlen]), (h, w, isz)
         pos = 16 + zlen
         if not (pos < len(data) and data[pos] == 1):
-            return blobs
+            return
         (flen,) = struct.unpack_from("<H", data, pos + 1)
+        yield "format", data[pos + 3:pos + 3 + flen], None
         pos += 3 + flen
-        for _ in range(3):
+        for name in _PLANES:
             (zl,) = struct.unpack_from("<I", data, pos)
-            ph, pw = struct.unpack_from("<II", data, pos + 4 + zl)
-            blobs.append((data[pos + 4:pos + 4 + zl], ph * pw))
+            raw = inflate(data[pos + 4:pos + 4 + zl])
+            yield name, raw, struct.unpack_from("<II", data, pos + 4 + zl)
             pos += 12 + zl
-        return blobs
+
+    @staticmethod
+    def keyframe_blobs(data: bytes):
+        """[(zlib blob, most bytes it may inflate to)] for the frame and, YUV frames, the three planes, in payload order; the
+        bounds are h w itemsize 4 for the frame and ph pw for a plane.  Raises struct.error (or another exception) on a
+        truncated layout, as decompress_frame would reach it."""
+        return [(blob, math.prod(shape) * (4 if name == "frame" else 1))
+                for name, blob, shape in FixedVideoCompressor._parts(data, lambda blob: blob) if name != "format"]
 
     def build_frame(self, data: bytes, inflate):
         """decompress_frame with inflate(blob) in place of zlib.decompress: called for the frame blob, then for each plane blob,
         at the points of the parse where decompress_frame inflates them."""
-        h, w, isz = struct.unpack_from("<III", data, 0)
-        (zlen,) = struct.unpack_from("<I", data, 12)
-        pos = 16
-        raw = inflate(data[pos:pos + zlen])
-        pos += zlen
+        parts = self._parts(data, inflate)
+        _, raw, (h, w, isz) = next(parts)
         dtype = _DTYPES.get(isz, np.float32)
         gray = h * w * isz
         if len(raw) > gray and len(raw) % gray == 0:
             frame = np.frombuffer(raw, dtype=dtype).reshape((h, w, len(raw) // gray))
         else:
             frame = np.frombuffer(raw, dtype=dtype).reshape((h, w))
-        has_yuv = pos < len(data) and data[pos] == 1
-        pos += 1
-        if not has_yuv:
-            return frame
-        (flen,) = struct.unpack_from("<H", data, pos)
-        pos += 2
-        info = {"format": data[pos:pos + flen].decode("utf-8")}
-        pos += flen
-        for name in ("y_plane", "u_plane", "v_plane"):
-            (zl,) = struct.unpack_from("<I", data, pos)
-            pos += 4
-            plane_raw = inflate(data[pos:pos + zl])
-            pos += zl
-            ph, pw = struct.unpack_from("<II", data, pos)
-            pos += 8
-            info[name] = np.frombuffer(plane_raw, dtype=np.uint8).reshape((ph, pw))
-        return YUVFrame(frame, info)
+        info = {}
+        for name, raw, shape in parts:
+            info[name] = raw.decode("utf-8") if name == "format" else np.frombuffer(raw, dtype=np.uint8).reshape(shape)
+        return YUVFrame(frame, info) if info else frame
 
     def compress_video(self, frames) -> List[bytes]:                             # fvc:183-198
         return [self.compress_frame(f) for f in frames]

@@ -26,6 +26,8 @@ import os
 import struct
 import time
 import zlib
+from concurrent.futures import Future
+from functools import partial
 from typing import Dict, List, Optional, Tuple
 
 import numpy as np
@@ -173,6 +175,12 @@ class BloomFilterCompressor:
 
 def _frame_data(frame) -> np.ndarray:
     return frame.data if hasattr(frame, "yuv_info") else np.asarray(frame)
+
+
+def _done(value) -> Future:
+    f = Future()
+    f.set_result(value)
+    return f
 
 
 class VideoFrameCompressor:
@@ -439,37 +447,23 @@ class ImprovedVideoCompressor:
         return np.packbits(np.unpackbits(mask_row, bitorder="little")[:n]).tobytes()
 
     @staticmethod
-    def _choose_values(vz: bytes, dz: Optional[bytes]):
-        """-> (value stream, vmode): the residual stream `dz` when it is strictly shorter than the values' `vz`, else `vz`; vmode is
-        None (an 'RBF2' payload) when there is no residual stream."""
-        if dz is None:
-            return vz, None
-        return (dz, 1) if len(dz) < len(vz) else (vz, 0)
-
-    @staticmethod
-    def _choose_motion(vz: bytes, dz: bytes, mz: bytes, fz: bytes):
-        """-> (value stream, vmode, zlib'd field or None) of value_coding "motion": the cheapest of the values (len(vz)), the residuals
-        (len(dz)) and the motion residuals with their field (len(mz) + 4 + len(fz)); a tie goes to the lower vmode."""
-        costs = (len(vz), len(dz), len(mz) + 4 + len(fz))
+    def _choose(streams: List[bytes], fz: Optional[bytes]):
+        """-> (value stream, vmode, zlib'd field or None) from the zlib'd value streams of kinds 0 (values), 1 (residuals) and, for
+        value_coding "motion", 2 (motion residuals, which cost their length + 4 + len(fz)).  The strict minimum wins and a tie goes to
+        the lower vmode; vmode is None (an 'RBF2' payload) for value_coding "plain", whose one stream is kind 0."""
+        if len(streams) == 1:
+            return streams[0], None, None
+        costs = [len(z) + (4 + len(fz) if kind == 2 else 0) for kind, z in enumerate(streams)]
         vmode = costs.index(min(costs))
-        return (vz, dz, mz)[vmode], vmode, fz if vmode == 2 else None
+        return streams[vmode], vmode, fz if vmode == 2 else None
 
     @staticmethod
-    def _inter_payload(shape, itemsize, ch, r, bm_row, wt_row, mask_row, values, resids=None, mresids=None, field=None) -> bytes:
-        """Assemble one inter-frame payload (runs in a worker thread; the zlib calls release the GIL).  With `resids` (adaptive
-        value coding) both value streams are compressed and the shorter one is kept; with `mresids` and `field` as well (motion value
-        coding) the three options are costed by _choose_motion."""
-        vz = zlib.compress(values.tobytes(), 9)
-        dz = None if resids is None else zlib.compress(resids.tobytes(), 9)
-        fz = None
-        if mresids is not None:
-            vz, vmode, fz = ImprovedVideoCompressor._choose_motion(vz, dz, zlib.compress(mresids.tobytes(), 9),
-                                                                   zlib.compress(field.tobytes(), 9))
-        else:
-            vz, vmode = ImprovedVideoCompressor._choose_values(vz, dz)
-        rz = zlib.compress(ImprovedVideoCompressor._raw_mask_bits(shape, mask_row), 9) if r.raw else None
-        return ImprovedVideoCompressor._inter_layout(shape, itemsize, ch, r, bm_row, wt_row, rz, vz, values.size, vmode, fz,
-                                                     mresids is not None)
+    def _inter_payload(shape, itemsize, ch, r, bm_row, wt_row, rz, streams, fz) -> bytes:
+        """One inter-frame payload from the futures of its zlib'd raw mask (raw pairs only), value streams (one per value kind) and
+        motion field (value_coding "motion" only).  Runs as a pool job submitted after those futures."""
+        vz, vmode, fz = ImprovedVideoCompressor._choose([s.result() for s in streams], None if fz is None else fz.result())
+        return ImprovedVideoCompressor._inter_layout(shape, itemsize, ch, r, bm_row, wt_row, None if rz is None else rz.result(), vz,
+                                                     r.ones * ch, vmode, fz, len(streams) == 3)
 
     @staticmethod
     def _inter_layout(shape, itemsize, ch, r, bm_row, wt_row, rz, vz, vcount, vmode=None, fz=None, v4=False) -> bytes:
@@ -536,6 +530,7 @@ class ImprovedVideoCompressor:
         shape, dtype = datas[0].shape, datas[0].dtype
         ch = shape[2] if len(shape) == 3 else 1
         group = max(2, int(self.batch_size))
+        kinds = {"plain": 1, "adaptive": 2, "motion": 3}[self.value_coding]      # value kinds 0 .. kinds-1 (_value_streams)
         st = FrameStream(shape[0], shape[1], ch, dtype, max_frames=2 * group, max_pairs=group,
                          mask_mode=1 if self.inter_frame_mode == "lossless" else 0)
         try:
@@ -547,76 +542,58 @@ class ImprovedVideoCompressor:
                 res = st.encode([slot[i - 1] for i in idxs], [slot[i] for i in idxs], float(self.inter_frame_threshold))
                 any_raw = any(r.raw for r in res)
                 bms, wts, masks = st.fetch_batch(0, len(idxs), want_masks=any_raw)   # one D2H per kind, one sync per group
-                if self.entropy_coder == "gpu":
-                    self._gpu_inter_payloads(st, shape, dtype.itemsize, ch, idxs, res, bms, wts, masks, out, pool)
-                    continue
-                gathered = st.gather_changed(len(idxs))            # N1: changed values of every pair, one launch, one copy
-                resids = self._with_residuals(st, st.gather_changed, len(idxs)) if self.value_coding != "plain" else None
-                fields, mres = self._with_motion(st, st.gather_changed, len(idxs)) if self.value_coding == "motion" else (None, None)
-                for j, i in enumerate(idxs):
-                    r = res[j]
-                    if r.resid and self.inter_frame_mode != "lossless":
-                        out[i] = None                              # not exactly representable: keyframe instead
-                        continue
-                    out[i] = pool.submit(self._inter_payload, shape, dtype.itemsize, ch, r, bms[j], wts[j],
-                                         masks[j] if (masks is not None and r.raw) else None, gathered[j],
-                                         None if resids is None else resids[j], None if mres is None else mres[j],
-                                         None if fields is None else fields[j])
+                # the pairs coded as inter frames; the others are not exactly representable: keyframes instead
+                keep = [j for j, r in enumerate(res) if not (r.resid and self.inter_frame_mode != "lossless")]
+                streams, fields = [], None
+                for kind in range(kinds):
+                    if kind == 2:
+                        fields = st.motion_search()
+                    streams.append(self._value_streams(st, kind, keep, pool))
+                raw = [j for j in keep if res[j].raw]
+                rzs = dict(zip(raw, self._zlib(pool, [masks[j] for j in raw], partial(self._raw_mask_bits, shape))))
+                fzs = self._zlib(pool, [fields[j] for j in keep]) if fields is not None else None
+                out.update(dict.fromkeys(idxs))
+                for k, j in enumerate(keep):
+                    out[idxs[j]] = pool.submit(self._inter_payload, shape, dtype.itemsize, ch, res[j], bms[j], wts[j], rzs.get(j),
+                                               [s[k] for s in streams], None if fzs is None else fzs[k])
         finally:
             st.close()
         return out
 
-    @staticmethod
-    def _with_residuals(st: FrameStream, fn, pairs: int):
-        """fn(pairs) with the stream's gathers returning residuals (value_mode 1) instead of the current samples."""
-        st.set_option("value_mode", 1)
+    def _value_streams(self, st: FrameStream, kind: int, keep: List[int], pool) -> List[Future]:
+        """Futures of the zlib'd value streams of the encoded pairs `keep`, gathered as value kind `kind`: 0 the current samples,
+        1 their residuals against the previous frame (value_mode 1), 2 the residuals against the motion-compensated previous frame
+        of the last motion_search (motion_values 1)."""
+        option = (None, "value_mode", "motion_values")[kind]
+        if option is None:
+            return self._zlib(pool, keep, st=st)
+        st.set_option(option, 1)
         try:
-            return fn(pairs)
+            return self._zlib(pool, keep, st=st)
         finally:
-            st.set_option("value_mode", 0)
+            st.set_option(option, 0)
 
-    @staticmethod
-    def _with_motion(st: FrameStream, fn, pairs: int):
-        """(the block motion fields of the encoded pairs, fn(pairs) with the stream's gathers returning residuals against the
-        motion-compensated previous frames (motion_values 1))."""
-        fields = st.motion_search(pairs)
-        st.set_option("motion_values", 1)
-        try:
-            return fields, fn(pairs)
-        finally:
-            st.set_option("motion_values", 0)
-
-    def _gpu_inter_payloads(self, st, shape, itemsize, ch, idxs, res, bms, wts, masks, out, pool) -> None:
-        """entropy_coder "gpu": changed values (and, adaptive or motion, their residuals) deflated where they were gathered (N1 + N4),
-        raw masks and motion fields in one batch each."""
-        n = len(idxs)
-        vzs = st.zlib_changed(n)
-        dzs = self._with_residuals(st, st.zlib_changed, n) if self.value_coding != "plain" else [None] * n
-        fields, mzs = self._with_motion(st, st.zlib_changed, n) if self.value_coding == "motion" else (None, None)
-        voffs = st.changed_offsets(n)
-        keep = [j for j, i in enumerate(idxs) if not (res[j].resid and self.inter_frame_mode != "lossless")]
-        raw_js = [j for j in keep if res[j].raw]
-        rzs = dict(zip(raw_js, deflate.compress_many([self._raw_mask_bits(shape, masks[j]) for j in raw_js])))
-        fzs = dict(zip(keep, deflate.compress_many([fields[j].tobytes() for j in keep]))) if fields is not None else {}
-        for j, i in enumerate(idxs):
-            if j not in keep:
-                out[i] = None                                      # not exactly representable: keyframe instead
-                continue
-            vcount = int(voffs[j + 1] - voffs[j]) // itemsize
-            fz = None
-            if mzs is not None:
-                vz, vmode, fz = self._choose_motion(vzs[j], dzs[j], mzs[j], fzs[j])
+    def _zlib(self, pool, items, make=lambda buf: buf, st: Optional[FrameStream] = None) -> List[Future]:
+        """Futures of zlib streams, one per item: of the buffer make(item), or with `st`, of the changed values of its encoded pair
+        `item` (all of its pairs are gathered).  This is the one step where the entropy coders differ.  "zlib": the host gathers the
+        values, and each make(item) with its level-9 zlib.compress runs as a job of `pool`.  "gpu": one device batch now, the values
+        deflated where zlib_changed gathers them."""
+        if self.entropy_coder == "gpu":
+            if st is not None:
+                zs = st.zlib_changed()
+                zs = [zs[j] for j in items]
             else:
-                vz, vmode = self._choose_values(vzs[j], dzs[j])
-            out[i] = pool.submit(self._inter_layout, shape, itemsize, ch, res[j], bms[j], wts[j], rzs.get(j), vz, vcount, vmode, fz,
-                                 mzs is not None)
+                zs = deflate.compress_many([make(x) for x in items])
+            return [_done(z) for z in zs]
+        if st is not None:
+            vals = st.gather_changed()                     # N1: changed values of every pair, one launch, one copy
+            items = [vals[j] for j in items]
+        return [pool.submit(lambda x: zlib.compress(make(x), 9), x) for x in items]
 
     def _keyframe_job(self, frame, pool):
-        """Callable returning the keyframe payload of `frame`: zlib level 9 in the pool, or coded on the GPU now."""
-        if self.entropy_coder == "gpu":
-            payload = assemble_keyframe(frame, deflate.compress_many(keyframe_raws(frame)))
-            return lambda: payload
-        return self.compressor.compress_frame_async(frame, pool)
+        """Callable returning the keyframe payload of `frame`, whose blobs _zlib codes."""
+        zs = self._zlib(pool, keyframe_raws(frame))
+        return lambda: assemble_keyframe(frame, [z.result() for z in zs])
 
     def compress_video(self, frames: List[np.ndarray], output_path: str = None, input_color_space: str = "BGR") -> Dict:
         if self.entropy_coder not in ("zlib", "gpu"):

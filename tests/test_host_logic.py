@@ -50,19 +50,23 @@ def test_shard_partition():
             assert max(sizes) - min(sizes) <= 1
 
 
-def test_keyframe_async_assembly_equals_serial():
-    """The GOP loop compresses a keyframe's zlib blobs as separate pool jobs: the assembled payload is byte-identical."""
+def test_keyframe_job_equals_compress_frame():
+    """The GOP loop compresses a keyframe's zlib blobs as separate pool jobs (ImprovedVideoCompressor._keyframe_job with the
+    "zlib" coder): the assembled payload is byte-identical to compress_frame's."""
     from concurrent.futures import ThreadPoolExecutor
     from new_bloom_filter_repo_b200.fixed_video_compressor import FixedVideoCompressor
+    from new_bloom_filter_repo_b200.improved_video_compressor import ImprovedVideoCompressor
     c = FixedVideoCompressor(verbose=False)
+    comp = object.__new__(ImprovedVideoCompressor)         # the "zlib" coder's keyframe job needs no device
+    comp.entropy_coder = "zlib"
     rng = np.random.default_rng(0)
     with ThreadPoolExecutor(3) as pool:
         for shape, dt in (((48, 64, 3), np.uint8), ((32, 40), np.uint8), ((20, 24, 3), np.uint16)):
             f = rng.integers(0, 200, shape).astype(dt)
-            assert c.compress_frame_async(f, pool)() == c.compress_frame(f)
+            assert comp._keyframe_job(f, pool)() == c.compress_frame(f)
             if f.ndim == 3:
                 y = c.add_yuv_info_to_frame(f)
-                assert c.compress_frame_async(y, pool)() == c.compress_frame(y)
+                assert comp._keyframe_job(y, pool)() == c.compress_frame(y)
 
 
 def test_bench_counters_go_stale_with_the_sources(tmp_path, monkeypatch):
