@@ -75,7 +75,7 @@ int rbf_device_info(rbf_ctx* ctx, char* name, int name_len, int* sm_count, int* 
                     uint64_t* total_mem_bytes);
 /* options: "k1_variant" (0 = vectorised loads, 1 = TMA bulk-copy ring), "query_smem_bytes" (cap), "query_variant",
  * "insert_variant", "host_chunk_frames", "encode_ranges" (1..8: K1/K2 pipelining depth of rbf_stream_encode),
- * "k1_ctas_per_sm" / "pipe_k1_ctas_per_sm" (K1 grid caps); "k1_only" / "mask_mode" here are only the defaults that
+ * "pipe_k1_sms" (the SMs its K1 runs on beside K2), "k1_ctas_per_sm" (K1 grid cap); "k1_only" / "mask_mode" here are only the defaults that
  * streams created afterwards inherit -- per-stream state lives in rbf_stream_set_option. */
 int rbf_set_option(rbf_ctx* ctx, const char* key, int64_t value);
 int64_t rbf_get_counter(rbf_ctx* ctx, const char* key);   /* "kernel_launches", "h2d_bytes", "d2h_bytes" */

@@ -182,7 +182,7 @@ def ctx():
                 h = C.c_void_p()
                 check(lib().rbf_ctx_create(dev, C.byref(h)))
                 _ctx = h
-                for key in ("query_variant", "insert_variant", "k1_variant", "encode_ranges", "pipe_k1_ctas_per_sm"):      # experiment knobs, e.g. RBF_QUERY_VARIANT=4
+                for key in ("query_variant", "insert_variant", "k1_variant", "encode_ranges", "pipe_k1_sms"):      # experiment knobs, e.g. RBF_QUERY_VARIANT=4
                     val = os.environ.get("RBF_" + key.upper())
                     if val is not None:
                         check(lib().rbf_set_option(h, key.encode(), int(val)), h)

@@ -41,8 +41,9 @@ struct rbf_ctx {
     cudaStream_t st_k1 = nullptr;     // pipelined encode: K1 of the later ranges + the witness memset run here, beside K2 on `st`
     cudaStream_t st_d2h = nullptr;    // rbf_stream_encode_host: result copies of chunk i overlap the kernels of chunk i+1
     cudaEvent_t ev_fork = nullptr, ev_wit = nullptr, ev_k1[8] = {nullptr}, ev_d2h = nullptr;
-    int encode_ranges = 1;            // rbf_stream_encode: K1/K2 pipelined over this many ranges of pairs (1 = serial, the default; a K2 CTA
-                                      // takes a whole SM's shared memory, so K1 and K2 overlap on different SMs)
+    int encode_ranges = 2;            // rbf_stream_encode: K1/K2 pipelined over this many ranges of pairs (1 = serial; see
+                                      // stream_encode_pipelined)
+    int pipe_k1_sms = 66;             // the SMs K1 of ranges 1.. runs on; K2 of the range before runs on the others
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaDeviceProp prop;
     LaunchCfg L;            // launcher options and the kernel counter
@@ -275,7 +276,7 @@ extern "C" int rbf_set_option(rbf_ctx* c, const char* key, int64_t v) {
     if (!strcmp(key, "kq_ranges")) { c->kq_ranges = (int)(v < 1 ? 1 : (v > 8 ? 8 : v)); return RBF_OK; }
     if (!strcmp(key, "encode_ranges")) { c->encode_ranges = (int)(v < 1 ? 1 : (v > 8 ? 8 : v)); return RBF_OK; }
     if (!strcmp(key, "k1_ctas_per_sm")) { c->L.k1_ctas_per_sm = (int)(v < 1 ? 1 : (v > 64 ? 64 : v)); return RBF_OK; }
-    if (!strcmp(key, "pipe_k1_ctas_per_sm")) { c->L.pipe_k1_ctas_per_sm = (int)(v < 1 ? 1 : (v > 64 ? 64 : v)); return RBF_OK; }
+    if (!strcmp(key, "pipe_k1_sms")) { c->pipe_k1_sms = (int)(v < 1 ? 1 : (v > 1024 ? 1024 : v)); return RBF_OK; }
     if (!strcmp(key, "query_smem_bytes")) {
         c->L.query_smem_cap = (int)((v <= 0 || v > query_max_smem_bytes()) ? query_max_smem_bytes() : v);
         return RBF_OK;
@@ -525,7 +526,7 @@ extern "C" int rbf_compress_mask(rbf_ctx* c, const uint8_t* mask, uint64_t n, co
     CK(c, cudaMemcpyAsync(d_prefix, h_prefix, 8, cudaMemcpyHostToDevice, c->st));
     CK(c, cudaMemsetAsync(d_bits, 0, bit_words_padded(l) * 4, c->st));
     CK(c, cudaMemsetAsync(d_wit, 0, mw * 4, c->st));
-    CK(c, launch_insert(c->L, d_job, 1, ncent, (uint32_t)l, c->st));
+    CK(c, launch_insert(c->L, d_job, 1, ncent, (uint32_t)l, c->L.sm_count, c->st));
     CK(c, launch_query(c->L, d_job, d_prefix, 1, ncent, (uint32_t)l, c->st));
     CK(c, launch_witness(c->L, d_job, 1, ncent, (uint32_t*)((uint8_t*)d_small + 1024), d_cnt + 1, c->st));
     CK(c, cudaMemcpyAsync(h_cnt, d_cnt, 16, cudaMemcpyDeviceToHost, c->st)); c->d2h += 16;
@@ -776,11 +777,11 @@ static bool pairs_form_chain(const PairJob* h, uint32_t count) {
     return true;
 }
 
-// K1 over pairs [f, f+cnt) on `st`, then the copy of their counts to the host.  pipelined: K2 runs beside it.
-static int enc_k1(rbf_stream* s, uint32_t f, uint32_t cnt, int thr_int, bool pipelined, cudaStream_t st) {
+// K1 over pairs [f, f+cnt) on `st`, then the copy of their counts to the host.  sms > 0: on that many SMs, K2 runs beside it.
+static int enc_k1(rbf_stream* s, uint32_t f, uint32_t cnt, int thr_int, int sms, cudaStream_t st) {
     rbf_ctx* c = s->c;
     CK(c, launch_threshold(c->L, s->d_pairs + f, (int)cnt, (uint32_t)s->npix, (int)s->C, (int)s->S, thr_int, s->mask_mode, s->gray_mode,
-                           s->d_ones + f, s->d_resid + f, pairs_form_chain(s->h_pairs + f, cnt), pipelined, st));
+                           s->d_ones + f, s->d_resid + f, pairs_form_chain(s->h_pairs + f, cnt), sms, st));
     CK(c, cudaMemcpyAsync(s->h_ones + f, s->d_ones + f, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, st));
     CK(c, cudaMemcpyAsync(s->h_resid + f, s->d_resid + f, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, st));
     c->d2h += 8 * (int64_t)cnt;
@@ -903,14 +904,14 @@ static int stream_encode_range(rbf_stream* s, uint32_t first, uint32_t count, ui
                                const uint32_t* curr_idx, int thr_int, const rbf_seeds* sd) {
     rbf_ctx* c = s->c;
     if (int r = enc_stage_pairs(s, first, count, prev_idx, curr_idx)) return r;
-    if (int r = enc_k1(s, first, count, thr_int, false, c->st)) return r;
+    if (int r = enc_k1(s, first, count, thr_int, 0, c->st)) return r;
     CK(c, cudaStreamSynchronize(c->st));               // the one host round trip: (p, k, l, T) need libm's log2
     RangeTotals rt;
     uint32_t* hp = s->h_prefix + pfx;
     stream_range_params(s, first, count, sd, nullptr, nullptr, hp, 0, &rt);
     if (int r = enc_stage_jobs(s, first, count, rt.max_l, hp)) return r;   // also when all raw: the caller copies these rows out
     if (rt.coded_pairs == 0) return RBF_OK;
-    CK(c, launch_insert(c->L, s->d_jobs + first, (int)count, (uint32_t)((s->npix + 99) / 100), rt.max_l, c->st));
+    CK(c, launch_insert(c->L, s->d_jobs + first, (int)count, (uint32_t)((s->npix + 99) / 100), rt.max_l, c->L.sm_count, c->st));
     CK(c, launch_query(c->L, s->d_jobs + first, s->d_prefix + pfx, (int)count, rt.total_cent, rt.max_l, c->st));
     return enc_witness(s, first, count, false);
 }
@@ -924,10 +925,12 @@ static int ensure_pipe_streams(rbf_ctx* c) {
     return RBF_OK;
 }
 
-// The resident-stream encode, pipelined: K1 has no host dependency, so K1 of ALL ranges is enqueued up front on a second
-// stream; as soon as a range's counts have landed the host derives its (k, l, T) and enqueues that range's K2 on the main
-// stream, where it can run beside K1 of the later ranges (K1 is HBM-bound with a grid that leaves SM slots free; K2's CTAs
-// take a whole SM's shared memory, so they start on SMs K1 leaves free), and the host round trip is hidden behind both.
+// The resident-stream encode, pipelined over R ranges of pairs: K1 has no host dependency, so K1 of ALL ranges is enqueued up
+// front on a second stream.  K1 of range 0 takes the whole GPU.  K1 of ranges 1.. runs on pipe_k1_sms SMs only, in CTAs whose
+// shared memory keeps K2 off those SMs (over the whole GPU K1 is HBM-bound; 66 of 132 SMs still pull 70 % of that bandwidth,
+// DESIGN §4).  As soon as range
+// r's counts have landed, the host derives its (k, l, T) while K1 of range r+1 runs, and enqueues K2 of range r on the main
+// stream, sized for the SMs K1 leaves free; K2 of the last range has nothing beside it and gets every SM.
 // K3 and K3b are single launches over all pairs.
 static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t* prev_idx, const uint32_t* curr_idx,
                                    double threshold, const rbf_seeds* sd, const double* kov, const uint64_t* lov) {
@@ -937,6 +940,7 @@ static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t
     uint32_t R = (uint32_t)c->encode_ranges;
     if (R > 8u) R = 8u;
     if (pairs < 8u * R) R = 1u;                          // small jobs: nothing to hide behind
+    const int k1_sms = c->pipe_k1_sms < c->L.sm_count ? c->pipe_k1_sms : c->L.sm_count - 1;   // K1 beside K2
     if (int r = ensure_pipe_streams(c)) return r;
     if (int r = enc_stage_pairs(s, 0, pairs, prev_idx, curr_idx)) return r;
     enc_begin(s, sd);
@@ -946,7 +950,7 @@ static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t
     uint32_t lo[9];
     for (uint32_t r = 0; r <= R; r++) lo[r] = (uint32_t)(((uint64_t)pairs * r) / R);
     for (uint32_t r = 0; r < R; r++) {
-        if (int e = enc_k1(s, lo[r], lo[r + 1] - lo[r], thr_int, R > 1u, c->st_k1)) return e;
+        if (int e = enc_k1(s, lo[r], lo[r + 1] - lo[r], thr_int, r > 0 ? k1_sms : 0, c->st_k1)) return e;
         CK(c, cudaEventRecord(c->ev_k1[r], c->st_k1));
     }
     CK(c, cudaEventRecord(s->ev[1], c->st_k1));           // end of the last K1
@@ -974,7 +978,7 @@ static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t
         if (int e = enc_stage_jobs(s, f, cnt, rt.max_l, nullptr)) return e;   // the work list goes up once, for all ranges
         if (rt.coded_pairs == 0) continue;
         if (first_k2) { CK(c, cudaEventRecord(s->ev[2], c->st)); first_k2 = false; }
-        if (!kq) CK(c, launch_insert(c->L, s->d_jobs + f, (int)cnt, ncent, rt.max_l, c->st));
+        if (!kq) CK(c, launch_insert(c->L, s->d_jobs + f, (int)cnt, ncent, rt.max_l, r + 1 < R ? c->L.sm_count - k1_sms : c->L.sm_count, c->st));
     }
     if (s->k1_only || all.coded_pairs == 0) {
         CK(c, cudaStreamWaitEvent(c->st, c->ev_k1[R - 1], 0));
@@ -998,7 +1002,7 @@ static int stream_encode_pipelined(rbf_stream* s, uint32_t pairs, const uint32_t
         CK(c, cudaStreamWaitEvent(c->st_k1, c->ev_fork, 0));
         for (uint32_t q = 0; q < Q; q++) {
             const uint32_t f = qlo[q], cnt = qlo[q + 1] - qlo[q];
-            CK(c, launch_insert(c->L, s->d_jobs + f, (int)cnt, ncent, all.max_l, c->st_k1));
+            CK(c, launch_insert(c->L, s->d_jobs + f, (int)cnt, ncent, all.max_l, c->L.sm_count, c->st_k1));
             CK(c, cudaEventRecord(c->ev_k1[q], c->st_k1));
             CK(c, cudaStreamWaitEvent(c->st, c->ev_k1[q], 0));
             if (q == 0) CK(c, cudaEventRecord(s->ev[3], c->st));

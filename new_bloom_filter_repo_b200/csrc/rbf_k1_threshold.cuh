@@ -239,38 +239,50 @@ __global__ void __launch_bounds__(K1_THREADS) k_threshold(const PairJob* __restr
 // Ragged end: the bulk copy of the last tile of a frame is rounded down to 16 B, which still holds every whole 32-pixel word of
 // the tile (a word ends on a multiple of 32 B); the ragged last word of the frame (< 32 px) is read from global memory by
 // threshold_word_tail.  Mask words at or beyond ceil(npix/32) are not written.
+// A CTA runs blockDim.x / SW_THREADS such sweeps, each with its own ring, mbarriers, counts and named barrier, and nothing
+// shared between them: sweep g of CTA b takes tiles (b * G + g) + k * (gridDim.x * G).  Over the whole GPU the launcher
+// runs one sweep per CTA; beside K2 it runs wide CTAs on a few SMs (see launch_threshold_sweep_t).
 // ------------------------------------------------------------------------------------------
-constexpr int SW_THREADS = 128;
+constexpr int SW_THREADS = 128;                       // one sweep
 constexpr uint32_t SW_TILE_PX = 32u * SW_THREADS;     // 4096 px: 4 / 8 / 12 / 24 KB per frame tile at 1 / 2 / 3 / 6 B per pixel
 constexpr int SW_STAGES = 4;                          // frames t and t+1 are read while t+2 and t+3 are in flight
+constexpr int SW_MAX_SWEEPS = 4;                      // sweeps per CTA (named barriers 1..4)
+// shared memory of one sweep: its ring, then its SW_STAGES mbarriers and the per-warp counts of two frames (96 B)
+template <int PB>
+__host__ __device__ constexpr uint32_t sw_sweep_bytes() { return (uint32_t)SW_STAGES * SW_TILE_PX * PB + 128u; }
 
 template <int PB, int S, bool GRAY = false>
-__global__ void __launch_bounds__(SW_THREADS) k_threshold_sweep(const PairJob* __restrict__ pairs, uint32_t P, uint32_t npix, int thr,
-                                                                int any_mode, uint32_t* __restrict__ ones, uint32_t* __restrict__ resid) {
+__global__ void __launch_bounds__(SW_THREADS * SW_MAX_SWEEPS) k_threshold_sweep(const PairJob* __restrict__ pairs, uint32_t P,
+                                                                                uint32_t npix, int thr, int any_mode,
+                                                                                uint32_t* __restrict__ ones, uint32_t* __restrict__ resid) {
     static_assert(!GRAY || PB == 3 * S, "BGR->gray needs three samples per pixel");
     constexpr uint32_t SLOT = SW_TILE_PX * PB;
     constexpr int NWARP = SW_THREADS / 32;
-    extern __shared__ __align__(128) uint8_t ring[];                   // [SW_STAGES][SLOT]
-    __shared__ __align__(8) uint64_t full[SW_STAGES];
-    __shared__ uint32_t s_cnt[2][NWARP][2];                            // per-warp (ones, resid) of the last two frames
+    extern __shared__ __align__(128) uint8_t k1_sweeps[];             // [sweep][sw_sweep_bytes<PB>()]
+    const uint32_t g = __shfl_sync(0xffffffffu, threadIdx.x / SW_THREADS, 0);   // this thread's sweep (warp-uniform for the compiler)
+    const uint32_t tid = threadIdx.x % SW_THREADS, G = blockDim.x / SW_THREADS;
+    uint8_t* const ring = k1_sweeps + g * sw_sweep_bytes<PB>();       // [SW_STAGES][SLOT]
+    uint64_t* const full = reinterpret_cast<uint64_t*>(ring + SW_STAGES * SLOT);
+    uint32_t(*const s_cnt)[NWARP][2] = reinterpret_cast<uint32_t(*)[NWARP][2]>(full + SW_STAGES);   // [2][NWARP][ones, resid]
+    const uint32_t sweep = blockIdx.x * G + g, nsweeps = gridDim.x * G;
     const uint32_t nwords = (npix + 31u) >> 5;
     const uint32_t ntiles = (npix + SW_TILE_PX - 1u) / SW_TILE_PX;
-    const uint32_t my_tiles = blockIdx.x < ntiles ? (ntiles - 1u - blockIdx.x) / gridDim.x + 1u : 0u;
+    const uint32_t my_tiles = sweep < ntiles ? (ntiles - 1u - sweep) / nsweeps + 1u : 0u;
     const uint32_t nfr = P + 1u;                                       // frames of the chain
-    const uint64_t total = (uint64_t)my_tiles * nfr;                   // this CTA's (tile, frame) loads, tile-major
+    const uint64_t total = (uint64_t)my_tiles * nfr;                   // this sweep's (tile, frame) loads, tile-major
     const K1Thr t = k1_thr(thr, any_mode);
-    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    const uint32_t lane = tid & 31u, warp = tid >> 5;
 
-    if (threadIdx.x == 0) {
+    if (tid == 0) {
         for (int s = 0; s < SW_STAGES; s++) mbar_init(&full[s], 1);
         fence_mbar_init();
     }
     __syncthreads();
 
-    // load i = (k-th tile of this CTA, frame j) into slot i % SW_STAGES; one thread issues
+    // load i = (k-th tile of this sweep, frame j) into slot i % SW_STAGES; one thread issues
     auto issue = [&](uint64_t i) {
         const uint32_t k = (uint32_t)(i / nfr), j = (uint32_t)(i % nfr);
-        const uint32_t px0 = (blockIdx.x + k * gridDim.x) * SW_TILE_PX;
+        const uint32_t px0 = (sweep + k * nsweeps) * SW_TILE_PX;
         const uint32_t tpx = npix - px0 < SW_TILE_PX ? npix - px0 : SW_TILE_PX;
         const uint32_t bytes = (tpx * PB) & ~15u;                      // whole 16 B units inside the frame
         const uint8_t* frame = j == 0 ? pairs[0].prev : pairs[j - 1].curr;
@@ -278,7 +290,7 @@ __global__ void __launch_bounds__(SW_THREADS) k_threshold_sweep(const PairJob* _
         mbar_expect_tx(bar, bytes);                                    // also the one arrival: a 0-byte load completes at once
         if (bytes) bulk_g2s(ring + (i % SW_STAGES) * SLOT, frame + (size_t)px0 * PB, bytes, bar);
     };
-    if (threadIdx.x == 0)
+    if (tid == 0)
         for (uint64_t i = 0; i < SW_STAGES - 1 && i < total; i++) issue(i);
 
     uint32_t k = 0, j = 0;                                             // tile and frame of load i
@@ -286,13 +298,13 @@ __global__ void __launch_bounds__(SW_THREADS) k_threshold_sweep(const PairJob* _
         mbar_wait(&full[i % SW_STAGES], (uint32_t)(i / SW_STAGES) & 1u);
         if (j > 0) {                                                   // pair j-1: frame j-1 (previous slot) against frame j
             const PairJob pj = pairs[j - 1];
-            const uint32_t w = (blockIdx.x + k * gridDim.x) * SW_THREADS + threadIdx.x;
+            const uint32_t w = (sweep + k * nsweeps) * SW_THREADS + tid;
             uint32_t m = 0, r = 0;
             if (w < nwords) {
                 const uint32_t px0 = w << 5;
                 if (px0 + 32u <= npix)
-                    threshold_word<PB, S, GRAY>(ring + ((i - 1) % SW_STAGES) * SLOT + threadIdx.x * 32u * PB,
-                                                ring + (i % SW_STAGES) * SLOT + threadIdx.x * 32u * PB, true, t, m, r);
+                    threshold_word<PB, S, GRAY>(ring + ((i - 1) % SW_STAGES) * SLOT + tid * 32u * PB,
+                                                ring + (i % SW_STAGES) * SLOT + tid * 32u * PB, true, t, m, r);
                 else
                     threshold_word_tail<PB, S, GRAY>(pj.prev + (size_t)px0 * PB, pj.curr + (size_t)px0 * PB, npix - px0, t, m, r);
                 pj.mask[w] = m;
@@ -300,8 +312,9 @@ __global__ void __launch_bounds__(SW_THREADS) k_threshold_sweep(const PairJob* _
             const uint32_t co = __reduce_add_sync(0xffffffffu, __popc(m)), cr = __reduce_add_sync(0xffffffffu, __popc(r));
             if (lane == 0) { s_cnt[i & 1][warp][0] = co; s_cnt[i & 1][warp][1] = cr; }
         }
-        __syncthreads();                                               // the previous slot has been read by every thread
-        if (threadIdx.x == 0) {
+        // the previous slot has been read by every thread of the sweep
+        asm volatile("bar.sync %0, %1;" ::"r"(g + 1u), "n"(SW_THREADS) : "memory");
+        if (tid == 0) {
             if (j > 0) {
                 uint32_t to = 0, tr = 0;
 #pragma unroll

@@ -127,31 +127,47 @@ static cudaError_t counted(LaunchCfg& L, int kernels = 1) {
     return cudaGetLastError();
 }
 
-// K1 over a chain of F >= 2 pairs: persistent CTAs, at most ctas_per_sm per SM, each sweeping the same number of tiles (or one fewer)
+// K1 over a chain of F >= 2 pairs: persistent sweeps, each of the same number of tiles (or one fewer).
+// sms == 0: the whole GPU, one sweep per CTA and at most ctas_per_sm CTAs per SM.
+// sms > 0: one wide CTA on each of `sms` SMs, with as many sweeps as fit in its shared memory (SW_MAX_SWEEPS at most).  Its
+// shared memory, padded to more than half an SM's 228 KB, keeps a second K1 CTA and any K2 CTA (195 KB) off the SM: the grid
+// lands on exactly that many SMs, and K2 runs beside it on the others.
 template <int PB, int S, bool GRAY>
 static cudaError_t launch_threshold_sweep_t(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t npix, int thr, int any_mode,
-                                            uint32_t* d_ones, uint32_t* d_resid, int ctas_per_sm, cudaStream_t st) {
-    const int smem = SW_STAGES * (int)SW_TILE_PX * PB;
-    cudaError_t e = cudaFuncSetAttribute(k_threshold_sweep<PB, S, GRAY>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+                                            uint32_t* d_ones, uint32_t* d_resid, int ctas_per_sm, int sms, cudaStream_t st) {
+    constexpr int sweep_smem = (int)sw_sweep_bytes<PB>();
+    constexpr int max_smem = 232448;                                   // opt-in shared memory of one CTA on sm_90
+    constexpr int wide = max_smem / sweep_smem < SW_MAX_SWEEPS ? max_smem / sweep_smem : SW_MAX_SWEEPS;
+    constexpr int wide_smem = wide * sweep_smem > max_smem / 2 + 1024 ? wide * sweep_smem : max_smem / 2 + 1024;
+    cudaError_t e = cudaFuncSetAttribute(k_threshold_sweep<PB, S, GRAY>, cudaFuncAttributeMaxDynamicSharedMemorySize, wide_smem);
     if (e != cudaSuccess) return e;
-    int per_sm = 1;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_threshold_sweep<PB, S, GRAY>, SW_THREADS, (size_t)smem);
-    if (e != cudaSuccess) return e;
-    const int cap = ctas_per_sm > 0 ? ctas_per_sm : 32;
-    if (per_sm > cap) per_sm = cap;
-    if (per_sm < 1) per_sm = 1;
     const uint32_t ntiles = (npix + SW_TILE_PX - 1u) / SW_TILE_PX;
-    const uint32_t slots = (uint32_t)(L.sm_count > 0 ? L.sm_count : 1) * (uint32_t)per_sm;
-    const uint32_t rounds = (ntiles + slots - 1u) / slots;
-    const uint32_t grid = (ntiles + rounds - 1u) / rounds;
-    k_threshold_sweep<PB, S, GRAY><<<grid, SW_THREADS, smem, st>>>(d_pairs, (uint32_t)F, npix, thr, any_mode, d_ones, d_resid);
+    uint32_t grid, sweeps = 1;
+    int smem = sweep_smem;
+    if (sms > 0) {
+        sweeps = (uint32_t)wide;
+        smem = wide_smem;
+        grid = (ntiles + sweeps - 1u) / sweeps;
+        if (grid > (uint32_t)sms) grid = (uint32_t)sms;
+    } else {
+        int per_sm = 1;
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_threshold_sweep<PB, S, GRAY>, SW_THREADS, (size_t)sweep_smem);
+        if (e != cudaSuccess) return e;
+        const int cap = ctas_per_sm > 0 ? ctas_per_sm : 32;
+        if (per_sm > cap) per_sm = cap;
+        if (per_sm < 1) per_sm = 1;
+        const uint32_t slots = (uint32_t)(L.sm_count > 0 ? L.sm_count : 1) * (uint32_t)per_sm;
+        const uint32_t rounds = (ntiles + slots - 1u) / slots;
+        grid = (ntiles + rounds - 1u) / rounds;
+    }
+    k_threshold_sweep<PB, S, GRAY><<<grid, SW_THREADS * sweeps, smem, st>>>(d_pairs, (uint32_t)F, npix, thr, any_mode, d_ones, d_resid);
     return counted(L);
 }
 
 // GRAY: the mask is taken on cv2.COLOR_BGR2GRAY of the three samples instead of on sample 0 (ivc:792-795); no TMA kernel for it
 template <int PB, int S, bool GRAY>
 static cudaError_t launch_threshold_t(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t npix, int thr, int any_mode, uint32_t* d_ones,
-                                      uint32_t* d_resid, bool chain, int ctas_per_sm, cudaStream_t st) {
+                                      uint32_t* d_resid, bool chain, int ctas_per_sm, int sms, cudaStream_t st) {
     const uint32_t nwords = (npix + 31u) >> 5;
     constexpr uint32_t TP = TMA_TILE_BYTES / PB;
     if constexpr (!GRAY) {
@@ -174,7 +190,7 @@ static cudaError_t launch_threshold_t(LaunchCfg& L, const PairJob* d_pairs, int 
             return cudaSuccess;
         }
     }
-    if (chain && F >= 2) return launch_threshold_sweep_t<PB, S, GRAY>(L, d_pairs, F, npix, thr, any_mode, d_ones, d_resid, ctas_per_sm, st);
+    if (chain && F >= 2) return launch_threshold_sweep_t<PB, S, GRAY>(L, d_pairs, F, npix, thr, any_mode, d_ones, d_resid, ctas_per_sm, sms, st);
     uint32_t bx = (nwords + 255u) / 256u;
     const uint32_t cap = (uint32_t)(L.sm_count * (ctas_per_sm > 0 ? ctas_per_sm : 32));
     if ((uint64_t)bx * (uint64_t)F > cap) { bx = (cap + (uint32_t)F - 1u) / (uint32_t)F; if (bx < 1u) bx = 1u; }
@@ -187,19 +203,20 @@ static cudaError_t launch_threshold_t(LaunchCfg& L, const PairJob* d_pairs, int 
 }
 
 cudaError_t launch_threshold(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t npix, int channels, int sample_bytes, int thr_int,
-                             int any_mode, int gray_mode, uint32_t* d_ones, uint32_t* d_resid, bool chain, bool pipelined,
-                             cudaStream_t st) {
+                             int any_mode, int gray_mode, uint32_t* d_ones, uint32_t* d_resid, bool chain, int sms, cudaStream_t st) {
     if (F <= 0 || npix == 0) return cudaSuccess;
-    const int pb = channels * sample_bytes, cap = pipelined ? L.pipe_k1_ctas_per_sm : L.k1_ctas_per_sm;
+    const int pb = channels * sample_bytes, cap = L.k1_ctas_per_sm;
+#define RBF_K1(PB_, S_, GRAY_) launch_threshold_t<PB_, S_, GRAY_>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, sms, st)
     if (gray_mode) {
-        if (pb == 3 && sample_bytes == 1) return launch_threshold_t<3, 1, true>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, st);
-        if (pb == 6 && sample_bytes == 2) return launch_threshold_t<6, 2, true>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, st);
+        if (pb == 3 && sample_bytes == 1) return RBF_K1(3, 1, true);
+        if (pb == 6 && sample_bytes == 2) return RBF_K1(6, 2, true);
         return cudaErrorInvalidValue;
     }
-    if (pb == 3 && sample_bytes == 1) return launch_threshold_t<3, 1, false>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, st);
-    if (pb == 6 && sample_bytes == 2) return launch_threshold_t<6, 2, false>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, st);
-    if (pb == 1 && sample_bytes == 1) return launch_threshold_t<1, 1, false>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, st);
-    if (pb == 2 && sample_bytes == 2) return launch_threshold_t<2, 2, false>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, st);
+    if (pb == 3 && sample_bytes == 1) return RBF_K1(3, 1, false);
+    if (pb == 6 && sample_bytes == 2) return RBF_K1(6, 2, false);
+    if (pb == 1 && sample_bytes == 1) return RBF_K1(1, 1, false);
+    if (pb == 2 && sample_bytes == 2) return RBF_K1(2, 2, false);
+#undef RBF_K1
     return cudaErrorInvalidValue;
 }
 
@@ -225,7 +242,7 @@ static cudaError_t insert_cluster_occupancy(uint32_t cs, int* clusters) {
     return cudaOccupancyMaxActiveClusters(clusters, k_insert_cluster, &cfg);
 }
 
-cudaError_t launch_insert(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t max_l_bits, cudaStream_t st) {
+cudaError_t launch_insert(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t max_l_bits, int sms, cudaStream_t st) {
     if (F <= 0 || max_centuries == 0) return cudaSuccess;
     const uint32_t words = (uint32_t)(((uint64_t)max_l_bits + 31u) >> 5);
     if (L.insert_variant >= 1 && words > 2u * K2_MAX_CS * K2_WORDS) {   // less than half of the array would be on chip: RED.OR into L2
@@ -239,13 +256,15 @@ cudaError_t launch_insert(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t 
         if (cs < 1u) cs = 1u;
         if (cs > (uint32_t)K2_MAX_CS) cs = K2_MAX_CS;    // the rest of the array is set with RED.OR in L2
         // Full waves of resident clusters take one frame each; the frames of the last, partial wave (all of them when F is small)
-        // get R copies each so that they still fill the GPU, with at least K2_WARPS slabs per CTA.
+        // get R copies each so that they still fill the `sms` SMs K2 has, with at least K2_WARPS slabs per CTA.
         if (L.k2_clusters[cs] == 0) {                       // first launch of this shape: measure it once, and refuse it if it does not fit
             cudaError_t e = insert_cluster_occupancy(cs, &L.k2_clusters[cs]);
             if (e != cudaSuccess) return e;
             if (L.k2_clusters[cs] < 1) { L.k2_clusters[cs] = 0; return cudaErrorInvalidConfiguration; }
         }
-        const uint32_t slots = (uint32_t)L.k2_clusters[cs], full = (uint32_t)F / slots * slots, rem = (uint32_t)F - full;
+        uint32_t slots = (uint32_t)((int64_t)L.k2_clusters[cs] * (sms < L.sm_count ? sms : L.sm_count) / L.sm_count);
+        if (slots < 1u) slots = 1u;
+        const uint32_t full = (uint32_t)F / slots * slots, rem = (uint32_t)F - full;
         const uint32_t nslab = (max_centuries + 31u) / 32u;
         const uint32_t useful = (nslab + cs * K2_WARPS - 1u) / (cs * K2_WARPS);
         uint32_t copies = rem ? slots / rem : 1u;

@@ -123,8 +123,7 @@ __host__ __device__ __forceinline__ void adler_combine(uint32_t& s1, uint32_t& s
 struct LaunchCfg {
     int sm_count = 0;
     int k1_variant = 0;
-    int k1_ctas_per_sm = 32;       // grid cap of K1 (pipelined encodes use pipe_k1_ctas_per_sm so that K2 finds room beside it)
-    int pipe_k1_ctas_per_sm = 4;
+    int k1_ctas_per_sm = 32;       // grid cap of K1 over the whole GPU
     int insert_variant = 1;        // 1: dense warp-compacted K2 building the arrays in shared memory (default); 0: per-lane K2, RED.OR into L2
     int query_variant = 5;         // 0: per-lane; 1: staged A->B->C rings, L2 tail; 2, 3, 4: as 5; 5: decade tiles with carried stage-B
                                    // batches (half tiles for 2^23 < m <= 2^24, ring kernel beyond); 6: half-decade tiles for every m <= 2^24
@@ -137,13 +136,15 @@ struct LaunchCfg {
 
 // launchers (all asynchronous on `st`); return cudaError_t of the launch
 // chain: the F pairs satisfy pairs[t].curr == pairs[t+1].prev and their frames are 16 B aligned (K1 then reads each frame once);
-// pipelined: K2 runs beside this K1, whose grid is then capped by L.pipe_k1_ctas_per_sm instead of L.k1_ctas_per_sm
+// sms > 0: a chain's K1 runs on exactly that many SMs, so that K2 runs beside it on the others (a pair list that is not a chain
+// takes the whole GPU whatever sms is); 0: the whole GPU, at most L.k1_ctas_per_sm CTAs per SM
 cudaError_t launch_threshold(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t npix, int channels, int sample_bytes,
-                             int thr_int, int any_mode, int gray_mode, uint32_t* d_ones, uint32_t* d_resid, bool chain, bool pipelined,
+                             int thr_int, int any_mode, int gray_mode, uint32_t* d_ones, uint32_t* d_resid, bool chain, int sms,
                              cudaStream_t st);
 // K2: variant 1 builds the arrays in (cluster) shared memory.  L.k2_clusters[1..8]: resident clusters of that many CTAs, 0 until
-// the first launch of the shape measures it with cudaOccupancyMaxActiveClusters (a shape that cannot be scheduled is an error)
-cudaError_t launch_insert(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t max_l_bits, cudaStream_t st);
+// the first launch of the shape measures it with cudaOccupancyMaxActiveClusters (a shape that cannot be scheduled is an error).
+// sms: the SMs K2 gets (L.sm_count, or fewer while K1 runs beside it); its waves are sized for that share of the clusters
+cudaError_t launch_insert(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t max_l_bits, int sms, cudaStream_t st);
 cudaError_t launch_query(LaunchCfg& L, const FrameJob* d_jobs, const uint32_t* d_cent_prefix, int F, uint32_t total_centuries,
                          uint32_t max_l_bits, cudaStream_t st);
 cudaError_t launch_witness(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t* d_scratch, uint32_t* d_wlen,

@@ -32,7 +32,7 @@ def main():
     bench.fill_stream(frames, seed=3, one_in=args.one_in)
     st = pkg.FrameStream(H, W, 3, np.uint8, max_frames=F)
     st.upload(frames)
-    base = {"query_variant": 5, "insert_variant": 1, "encode_ranges": 1, "pipe_k1_ctas_per_sm": 4, "query_smem_bytes": 0, "query_warps": 0, "kq_ranges": 1}
+    base = {"query_variant": 5, "insert_variant": 1, "encode_ranges": 1, "pipe_k1_sms": 66, "query_smem_bytes": 0, "query_warps": 0, "kq_ranges": 1}
     sweep = json.loads(args.configs) if args.configs else [
         {}, {"query_variant": 1}, {"query_variant": 6}, {"insert_variant": 0}, {"encode_ranges": 4},
         {"query_smem_bytes": 200000}, {"query_smem_bytes": 170000}, {"query_smem_bytes": 140000}, {"query_smem_bytes": 110000},
