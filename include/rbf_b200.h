@@ -194,12 +194,13 @@ int rbf_stream_stage_ms(rbf_stream* s, double out[6]);
  *     row-major order.  offsets_out[pairs+1] = byte offsets per pair; values_out == NULL only fills the offsets. */
 int rbf_stream_gather_changed(rbf_stream* s, uint32_t pairs, uint8_t* values_out, uint64_t values_capacity,
                               uint64_t* offsets_out);
-/* N2  VideoFrameCompressor._apply_frame_diff (ivc:849-909): store[out_frame] = store[base_frame] with the pixels selected
- *     by the mask (n bits, little bit order) replaced by `values` in rank order; when the value count does not match the
- *     mask the base frame is copied unchanged (ivc:882) and *applied_pixels = 0. */
-int rbf_stream_apply_diff(rbf_stream* s, uint32_t base_frame, uint32_t out_frame, const uint8_t* mask_packed_little,
-                          const uint8_t* values, uint64_t values_bytes, uint64_t* applied_pixels);
-int rbf_stream_download(rbf_stream* s, uint32_t frame, void* host_out);
+/* N2  VideoFrameCompressor._apply_frame_diff (ivc:849-909): frame (base_frame + 1) % max_frames = frame base_frame with the
+ *     pixels selected by the mask (n bits, little bit order) replaced by `values` in rank order -- rbf_stream_apply_chain of one
+ *     pair, with the mask and values from the host; when the value count does not match the mask the base frame is copied
+ *     unchanged (ivc:882) and *applied_pixels = 0.  One H2D copy each of the mask, the values and the offsets; one
+ *     synchronisation (two on a mismatch). */
+int rbf_stream_apply_diff(rbf_stream* s, uint32_t base_frame, const uint8_t* mask_packed_little, const uint8_t* values,
+                          uint64_t values_bytes, uint64_t* applied_pixels);
 /* ---- K4b / K4c: a group of inter frames decoded at once (ImprovedVideoCompressor.decompress_video)
  * rbf_stream_decode_masks  BloomFilterCompressor.decompress (ivc:268-307) of `count` pairs in one query + expand launch: pair i's
  *     payload bytes as stored, in slots like those of rbf_stream_fetch_batch -- bitmaps_packbits + i*bitmap_slot_bytes holds
@@ -230,7 +231,8 @@ int rbf_stream_download(rbf_stream* s, uint32_t frame, void* host_out);
  *     behind one tile count and scan for the whole chain on one CUDA stream.  Frame slots are taken modulo max_frames, so a
  *     chain may continue from the last frame of the previous one wherever it sits; count < max_frames.  ivc:882 per pair: pair
  *     i is applied only if its mask's popcount x pixel bytes equals its value bytes; the first pair that fails gets
- *     applied_out[i] = 0 and no frame from there on is written.  applied_out[i] = pixels applied.
+ *     applied_out[i] = 0 and no frame from there on is written.  applied_out[i] = pixels applied.  rbf_stream_apply_diff is
+ *     the same sweep over one pair.
  * rbf_stream_download_batch  frames first .. first+count-1 (slots modulo max_frames) into one contiguous host array, one
  *     synchronisation. */
 int rbf_stream_decode_masks(rbf_stream* s, uint32_t count, const uint8_t* bitmaps_packbits, uint64_t bitmap_slot_bytes,

@@ -48,7 +48,7 @@ EXPORTS = [
     "rbf_compress_mask", "rbf_decompress_mask",
     "rbf_stream_create", "rbf_stream_destroy", "rbf_stream_set_option", "rbf_stream_upload", "rbf_stream_frame_ptr", "rbf_stream_encode",
     "rbf_stream_encode_host", "rbf_stream_fetch", "rbf_stream_fetch_batch", "rbf_stream_decode_verify", "rbf_stream_bitmap_region", "rbf_stream_stage_ms",
-    "rbf_stream_gather_changed", "rbf_stream_apply_diff", "rbf_stream_download", "rbf_median_blur5", "rbf_stream_median5",
+    "rbf_stream_gather_changed", "rbf_stream_apply_diff", "rbf_median_blur5", "rbf_stream_median5",
     "rbf_stream_decode_masks", "rbf_stream_apply_chain", "rbf_stream_motion_search", "rbf_stream_download_batch",
     "rbf_zlib_bound", "rbf_deflate_code_lengths", "rbf_zlib_compress_batch", "rbf_stream_zlib_changed",
     "rbf_inflate_segment", "rbf_zlib_decompress_batch", "rbf_stream_inflate_values",
@@ -118,8 +118,7 @@ def _sig(L):
     L.rbf_stream_bitmap_region.argtypes = [vp, P(vp), P(u64)]
     L.rbf_stream_stage_ms.argtypes = [vp, vp]
     L.rbf_stream_gather_changed.argtypes = [vp, u32, vp, u64, vp]
-    L.rbf_stream_apply_diff.argtypes = [vp, u32, u32, vp, vp, u64, P(u64)]
-    L.rbf_stream_download.argtypes = [vp, u32, vp]
+    L.rbf_stream_apply_diff.argtypes = [vp, u32, vp, vp, u64, P(u64)]
     L.rbf_stream_decode_masks.argtypes = [vp, u32, vp, u64, vp, u64, vp, vp, vp, vp, P(Seeds), vp, vp]
     L.rbf_stream_apply_chain.argtypes = [vp, u32, u32, vp, vp, vp, vp, vp]
     L.rbf_stream_motion_search.argtypes = [vp, u32, vp]

@@ -87,8 +87,8 @@ enum ScratchSlot {
     kScrMask, kScrBits, kScrPass, kScrWit,        // the single-mask coder's FrameJob buffers
     kScrSmall,                                    // its counts, prefix and job; decode_verify's mismatch counts
     kScrValues,                                   // changed values: gather_changed, zlib_changed, apply_diff, apply_chain
-    kScrGatherJobs, kScrApplyMask, kScrMedianIn, kScrMedianOut,
-    kScrGatherCounts,                             // per-chunk set-bit counts of the gather / scatter kernels
+    kScrGatherJobs, kScrApplyMask, kScrMedianIn, kScrMedianOut,   // the gather's jobs, apply_diff's mask, median5 planes
+    kScrGatherCounts,                             // per-chunk set-bit counts of the gather
     kScrZlibRes, kScrZlibOut, kScrZlibStage, kScrZlibSegs, kScrZlibCopies, kScrZlibSmall, kScrZlibIn,
     kScrDecodeCounts, kScrChainSmall, kScrChainTiles,   // decode_masks' counts; apply_chain's offsets + flags + totals, tile prefix
     kScrInflateIn, kScrInflateSmall, kScrInflateSlots, kScrInflateRes, kScrInflateOut,   // inflate_streams / inflate_place
@@ -1204,15 +1204,14 @@ static int gather_values(rbf_stream* s, uint32_t pairs, const uint64_t* offs, ui
         J.frame = s->h_pairs[i].curr;
         J.prev = s->h_pairs[i].prev;
         J.values = (uint8_t*)d_vals + offs[i];
-        J.out_frame = nullptr;
         J.npix = (uint32_t)s->npix;
         J.pix_bytes = pb;
         J.width = s->W;
         J.field = s->motion_values ? s->d_fields + i * field_bytes : nullptr;
     }
     CK(c, cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(GatherJob) * pairs, cudaMemcpyHostToDevice, c->st));   // pageable: staged before return
-    CK(c, launch_gather_scatter(c->L, (const GatherJob*)d_jobs, (int)pairs, 0, (uint32_t)s->npix, pb, (uint32_t*)d_gcnt, nullptr, c->st,
-                                s->value_mode || s->motion_values ? s->S : 0u, s->motion_values != 0));
+    CK(c, launch_gather(c->L, (const GatherJob*)d_jobs, (int)pairs, (uint32_t)s->npix, pb, (uint32_t*)d_gcnt, c->st,
+                        s->value_mode || s->motion_values ? s->S : 0u, s->motion_values != 0));
     *d_values = (uint8_t*)d_vals;
     return RBF_OK;
 }
@@ -1229,54 +1228,6 @@ extern "C" int rbf_stream_gather_changed(rbf_stream* s, uint32_t pairs, uint8_t*
     uint8_t* d_vals;
     if (int r = gather_values(s, pairs, offsets_out, &d_vals)) return r;
     if (total) { CK(c, cudaMemcpyAsync(values_out, d_vals, (size_t)total, cudaMemcpyDeviceToHost, c->st)); c->d2h += (int64_t)total; }
-    CK(c, cudaStreamSynchronize(c->st));
-    return RBF_OK;
-}
-
-extern "C" int rbf_stream_apply_diff(rbf_stream* s, uint32_t base_frame, uint32_t out_frame, const uint8_t* mask_packed_little,
-                                     const uint8_t* values, uint64_t values_bytes, uint64_t* applied_pixels) {
-    if (!s || !mask_packed_little || (!values && values_bytes)) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_apply_diff: NULL");
-    rbf_ctx* c = s->c;
-    if (base_frame >= s->max_frames || out_frame >= s->max_frames) return set_err(c, RBF_ERR_INVALID, "frame index outside the store");
-    CK(c, cudaSetDevice(c->device));
-    const uint64_t pb = (uint64_t)s->C * s->S;
-    const size_t mbytes = (size_t)((s->npix + 7) / 8), mwords = s->mask_stride_w;
-    void *d_mask, *d_vals, *d_job, *d_gcnt;
-    int rc;
-    if ((rc = scratch_get(c, kScrApplyMask, mwords * 4, &d_mask)) || (rc = scratch_get(c, kScrValues, (size_t)values_bytes + 256, &d_vals)) ||
-        (rc = scratch_get(c, kScrGatherJobs, sizeof(GatherJob) + 64, &d_job)) ||
-        (rc = scratch_get(c, kScrGatherCounts, 4 * (size_t)gather_chunks((uint32_t)s->npix) + 64, &d_gcnt)))
-        return rc;
-    CK(c, cudaMemsetAsync(d_mask, 0, mwords * 4, c->st));
-    CK(c, cudaMemcpyAsync(d_mask, mask_packed_little, mbytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)mbytes;
-    if (values_bytes) { CK(c, cudaMemcpyAsync(d_vals, values, (size_t)values_bytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)values_bytes; }
-    uint8_t* dst = s->d_frames + (size_t)out_frame * s->frame_stride;
-    if (out_frame != base_frame)
-        CK(c, cudaMemcpyAsync(dst, s->d_frames + (size_t)base_frame * s->frame_stride, s->frame_bytes, cudaMemcpyDeviceToDevice, c->st));
-    GatherJob J;
-    J.mask = (const uint32_t*)d_mask; J.frame = nullptr; J.values = (uint8_t*)d_vals; J.out_frame = dst;
-    J.npix = (uint32_t)s->npix; J.pix_bytes = (uint32_t)pb; J.width = s->W; J.field = nullptr;
-    uint32_t* d_cnt = (uint32_t*)((uint8_t*)d_job + sizeof(GatherJob));
-    // the reference applies the diff only when the value count matches the mask (ivc:882): count first
-    CK(c, cudaMemsetAsync(d_cnt, 0, 4, c->st));
-    CK(c, launch_popcount(c->L, (const uint32_t*)d_mask, (s->npix + 31) / 32, d_cnt, c->st));
-    uint32_t h_cnt = 0;
-    CK(c, cudaMemcpyAsync(&h_cnt, d_cnt, 4, cudaMemcpyDeviceToHost, c->st));
-    CK(c, cudaStreamSynchronize(c->st));
-    if (applied_pixels) *applied_pixels = 0;
-    if ((uint64_t)h_cnt * pb != values_bytes) return RBF_OK;       // ivc:882: mismatch -> the base frame is returned unchanged
-    CK(c, cudaMemcpyAsync(d_job, &J, sizeof J, cudaMemcpyHostToDevice, c->st));
-    CK(c, launch_gather_scatter(c->L, (const GatherJob*)d_job, 1, 1, (uint32_t)s->npix, (uint32_t)pb, (uint32_t*)d_gcnt, nullptr, c->st));
-    CK(c, cudaStreamSynchronize(c->st));
-    if (applied_pixels) *applied_pixels = h_cnt;
-    return RBF_OK;
-}
-
-extern "C" int rbf_stream_download(rbf_stream* s, uint32_t frame, void* host_out) {
-    if (!s || !host_out || frame >= s->max_frames) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_download: bad argument");
-    rbf_ctx* c = s->c;
-    CK(c, cudaMemcpyAsync(host_out, s->d_frames + (size_t)frame * s->frame_stride, s->frame_bytes, cudaMemcpyDeviceToHost, c->st));
-    c->d2h += (int64_t)s->frame_bytes;
     CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
 }
@@ -1353,6 +1304,56 @@ extern "C" int rbf_stream_decode_masks(rbf_stream* s, uint32_t count, const uint
     return RBF_OK;
 }
 
+// K4c over pairs [0, count) from base_frame: pair i's mask at d_masks + i * mask_stride_w, its values at d_vals + value_offsets[i]
+// (device), modes / fields as in rbf_stream_apply_chain, already validated (field_bytes: 0 when no field is read).  One H2D copy of
+// the offsets with the modes and fields behind them, one synchronisation.  *first_bad_out (may be NULL): the first pair whose value
+// count does not match its mask (ivc:882), UINT32_MAX when none.
+static int stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* d_vals, const uint64_t* value_offsets,
+                              const uint8_t* modes, const int8_t* fields, size_t field_bytes, const uint32_t* d_masks,
+                              size_t mask_stride_w, uint64_t* applied_out, uint32_t* first_bad_out) {
+    rbf_ctx* c = s->c;
+    const uint32_t ntiles = (uint32_t)((s->npix + AP_TILE_PX - 1) / AP_TILE_PX);
+    void *d_small, *d_pfx;
+    int rc;
+    // d_small: the value offsets, then the modes, then the fields (one H2D copy for all three), then first_bad and the totals
+    const size_t off_bytes = 8 * ((size_t)count + 1), flag_bytes = modes ? count : 0;
+    const size_t res_at = align_up(off_bytes + flag_bytes + field_bytes, 16);
+    const size_t small = res_at + 4 * ((size_t)count + 1) + (field_bytes ? 4 * (size_t)count : 0);   // + the runs' first_bad words
+    if ((rc = scratch_get(c, kScrChainSmall, small, &d_small)) || (rc = scratch_get(c, kScrChainTiles, 4 * (size_t)count * ntiles, &d_pfx)))
+        return rc;
+    uint64_t* d_off = (uint64_t*)d_small;
+    uint32_t* d_res = (uint32_t*)((uint8_t*)d_small + res_at);   // [0] first_bad, [1 + i] totals
+    if (modes) {
+        std::vector<uint8_t> head(off_bytes + flag_bytes + field_bytes);
+        memcpy(head.data(), value_offsets, off_bytes);
+        memcpy(head.data() + off_bytes, modes, flag_bytes);
+        if (field_bytes) memcpy(head.data() + off_bytes + flag_bytes, fields, field_bytes);
+        CK(c, cudaMemcpyAsync(d_off, head.data(), head.size(), cudaMemcpyHostToDevice, c->st));   // pageable: staged before return
+    } else {
+        CK(c, cudaMemcpyAsync(d_off, value_offsets, off_bytes, cudaMemcpyHostToDevice, c->st));
+    }
+    c->h2d += (int64_t)(off_bytes + flag_bytes + field_bytes);
+    CK(c, cudaMemsetAsync(d_res, 0xff, 4, c->st));
+    ApplyChain A;
+    A.masks = d_masks; A.mask_stride_w = mask_stride_w;
+    A.frames = s->d_frames; A.frame_stride = s->frame_stride;
+    A.max_frames = s->max_frames; A.base = base_frame;
+    A.npix = (uint32_t)s->npix; A.ntiles = ntiles; A.count = count; A.pix_bytes = s->C * s->S;
+    A.values = d_vals; A.value_off = d_off;
+    A.sample_bytes = s->S;
+    A.tile_pfx = (uint32_t*)d_pfx; A.totals = d_res + 1; A.first_bad = d_res;
+    A.residual = modes ? (const uint8_t*)d_small + off_bytes : nullptr;     // read by runs with a mode-1 or mode-2 pair only
+    CK(c, launch_apply_chain(c->L, A, modes, field_bytes ? (const int8_t*)d_small + off_bytes + flag_bytes : nullptr, s->H, s->W,
+                             d_res + 1 + count, c->st));
+    std::vector<uint32_t> h((size_t)count + 1);
+    CK(c, cudaMemcpyAsync(h.data(), d_res, 4 * ((size_t)count + 1), cudaMemcpyDeviceToHost, c->st));
+    c->d2h += 4 * ((int64_t)count + 1);
+    CK(c, cudaStreamSynchronize(c->st));
+    for (uint32_t i = 0; i < count; i++) applied_out[i] = i < h[0] ? h[1 + i] : 0;
+    if (first_bad_out) *first_bad_out = h[0];
+    return RBF_OK;
+}
+
 extern "C" int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32_t count, const uint8_t* values,
                                       const uint64_t* value_offsets, const uint8_t* modes, const int8_t* fields, uint64_t* applied_out) {
     if (!s || !value_offsets || !applied_out) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_apply_chain: NULL");
@@ -1369,10 +1370,9 @@ extern "C" int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32
                        base_frame, s->max_frames, s->max_pairs);
     for (uint32_t i = 0; i < count; i++)
         if (value_offsets[i + 1] < value_offsets[i]) return set_err(c, RBF_ERR_INVALID, "value offsets decrease at pair %u", i);
-    bool any_residual = false, any_motion = false;
+    bool any_motion = false;
     for (uint32_t i = 0; modes && i < count; i++) {
         if (modes[i] > 2) return set_err(c, RBF_ERR_INVALID, "pair %u: value mode %u is not 0, 1 or 2", i, (unsigned)modes[i]);
-        any_residual |= modes[i] == 1;
         any_motion |= modes[i] == 2;
     }
     const size_t field_bytes = modes && fields ? (size_t)count * mv_blocks(s->H, s->W) * 2 : 0;
@@ -1382,47 +1382,43 @@ extern "C" int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32
             return set_err(c, RBF_ERR_INVALID, "pair %llu: motion vector component %d is outside [-%d, %d]",
                            (unsigned long long)(i / (field_bytes / count)), (int)fields[i], MV_RANGE, MV_RANGE);
     CK(c, cudaSetDevice(c->device));
-    const uint32_t ntiles = (uint32_t)((s->npix + AP_TILE_PX - 1) / AP_TILE_PX);
-    const bool on_device = !values && vbytes;            // the values are where rbf_stream_inflate_values left them
-    void *d_vals = s->d_inflated, *d_small, *d_pfx;
-    int rc;
-    // d_small: the value offsets, then the modes, then the fields (one H2D copy for all three), then first_bad and the totals
-    const size_t off_bytes = 8 * ((size_t)count + 1), flag_bytes = modes ? count : 0;
-    const size_t res_at = align_up(off_bytes + flag_bytes + field_bytes, 16);
-    const size_t small = res_at + 4 * ((size_t)count + 1) + (field_bytes ? 4 * (size_t)count : 0);   // + the runs' first_bad words
-    if ((!on_device && (rc = scratch_get(c, kScrValues, (size_t)vbytes + 256, &d_vals))) || (rc = scratch_get(c, kScrChainSmall, small, &d_small)) ||
-        (rc = scratch_get(c, kScrChainTiles, 4 * (size_t)count * ntiles, &d_pfx)))
-        return rc;
-    uint64_t* d_off = (uint64_t*)d_small;
-    uint32_t* d_res = (uint32_t*)((uint8_t*)d_small + res_at);   // [0] first_bad, [1 + i] totals
-    if (values && vbytes) { CK(c, cudaMemcpyAsync(d_vals, values, (size_t)vbytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)vbytes; }
-    if (modes) {
-        std::vector<uint8_t> head(off_bytes + flag_bytes + field_bytes);
-        memcpy(head.data(), value_offsets, off_bytes);
-        memcpy(head.data() + off_bytes, modes, flag_bytes);
-        if (field_bytes) memcpy(head.data() + off_bytes + flag_bytes, fields, field_bytes);
-        CK(c, cudaMemcpyAsync(d_off, head.data(), head.size(), cudaMemcpyHostToDevice, c->st));   // pageable: staged before return
-    } else {
-        CK(c, cudaMemcpyAsync(d_off, value_offsets, off_bytes, cudaMemcpyHostToDevice, c->st));
+    void* d_vals = s->d_inflated;
+    if (values || !vbytes) {                             // else the values are where rbf_stream_inflate_values left them
+        if (int r = scratch_get(c, kScrValues, (size_t)vbytes + 256, &d_vals)) return r;
+        if (vbytes) { CK(c, cudaMemcpyAsync(d_vals, values, (size_t)vbytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)vbytes; }
     }
-    c->h2d += (int64_t)(off_bytes + flag_bytes + field_bytes);
-    CK(c, cudaMemsetAsync(d_res, 0xff, 4, c->st));
-    ApplyChain A;
-    A.masks = s->d_mask; A.mask_stride_w = s->mask_stride_w;
-    A.frames = s->d_frames; A.frame_stride = s->frame_stride;
-    A.max_frames = s->max_frames; A.base = base_frame;
-    A.npix = (uint32_t)s->npix; A.ntiles = ntiles; A.count = count; A.pix_bytes = s->C * s->S;
-    A.values = (const uint8_t*)d_vals; A.value_off = d_off;
-    A.sample_bytes = s->S;
-    A.tile_pfx = (uint32_t*)d_pfx; A.totals = d_res + 1; A.first_bad = d_res;
-    A.residual = any_residual || any_motion ? (const uint8_t*)d_small + off_bytes : nullptr;
-    CK(c, launch_apply_chain(c->L, A, modes, field_bytes ? (const int8_t*)d_small + off_bytes + flag_bytes : nullptr, s->H, s->W,
-                             d_res + 1 + count, c->st));
-    std::vector<uint32_t> h((size_t)count + 1);
-    CK(c, cudaMemcpyAsync(h.data(), d_res, 4 * ((size_t)count + 1), cudaMemcpyDeviceToHost, c->st));
-    c->d2h += 4 * ((int64_t)count + 1);
-    CK(c, cudaStreamSynchronize(c->st));
-    for (uint32_t i = 0; i < count; i++) applied_out[i] = i < h[0] ? h[1 + i] : 0;
+    return stream_apply_chain(s, base_frame, count, (const uint8_t*)d_vals, value_offsets, modes, fields, field_bytes, s->d_mask,
+                              s->mask_stride_w, applied_out, nullptr);
+}
+
+// The one-pair chain from base_frame into frame (base_frame + 1) % max_frames, with the mask and values from the host
+extern "C" int rbf_stream_apply_diff(rbf_stream* s, uint32_t base_frame, const uint8_t* mask_packed_little, const uint8_t* values,
+                                     uint64_t values_bytes, uint64_t* applied_pixels) {
+    if (!s || !mask_packed_little || (!values && values_bytes)) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_apply_diff: NULL");
+    rbf_ctx* c = s->c;
+    if (base_frame >= s->max_frames) return set_err(c, RBF_ERR_INVALID, "frame index outside the store");
+    CK(c, cudaSetDevice(c->device));
+    const size_t mbytes = (size_t)((s->npix + 7) / 8), mwords = s->mask_stride_w;
+    void *d_mask, *d_vals;
+    int rc;
+    if ((rc = scratch_get(c, kScrApplyMask, mwords * 4, &d_mask)) || (rc = scratch_get(c, kScrValues, (size_t)values_bytes + 256, &d_vals)))
+        return rc;
+    CK(c, cudaMemsetAsync(d_mask, 0, mwords * 4, c->st));
+    CK(c, cudaMemcpyAsync(d_mask, mask_packed_little, mbytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)mbytes;
+    if (values_bytes) { CK(c, cudaMemcpyAsync(d_vals, values, (size_t)values_bytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)values_bytes; }
+    const uint64_t offs[2] = {0, values_bytes};
+    uint64_t applied = 0;
+    uint32_t first_bad = 0;
+    if (int r = stream_apply_chain(s, base_frame, 1, (const uint8_t*)d_vals, offs, nullptr, nullptr, 0, (const uint32_t*)d_mask, mwords,
+                                   &applied, &first_bad))
+        return r;
+    if (first_bad == 0) {                                // ivc:882: the sweep wrote nothing; the output is the base frame unchanged
+        const uint32_t out = base_frame + 1 == s->max_frames ? 0 : base_frame + 1;
+        CK(c, cudaMemcpyAsync(s->d_frames + (size_t)out * s->frame_stride, s->d_frames + (size_t)base_frame * s->frame_stride,
+                              s->frame_bytes, cudaMemcpyDeviceToDevice, c->st));
+        CK(c, cudaStreamSynchronize(c->st));
+    }
+    if (applied_pixels) *applied_pixels = applied;
     return RBF_OK;
 }
 

@@ -1,9 +1,9 @@
-// rbf_aux_kernels.cuh -- N1/N2 gather + scatter (ivc:810-909), N3 5x5 median (ivc:738), bit packing utilities, explicit item lists (ivc:99-138, rbf:25-182).  Included by rbf_kernels.cu inside namespace rbf.
+// rbf_aux_kernels.cuh -- N1 gather (ivc:810-842), N3 5x5 median (ivc:738), bit packing utilities, explicit item lists (ivc:99-138, rbf:25-182).  Included by rbf_kernels.cu inside namespace rbf.
 #pragma once
 
 // ------------------------------------------------------------------------------------------
-// N1 / N2 (SURVEY 8f): ordered gather of the changed pixels' values (ivc:810-842) and the scatter
-// that rebuilds the next frame (ivc:849-909).  A pair is cut into `chunks` runs of mask words; a
+// N1 (SURVEY 8f): ordered gather of the changed pixels' values (ivc:810-842); N2, the frame rebuilt
+// from them, is the K4c sweep (rbf_k4c_apply.cuh).  A pair is cut into `chunks` runs of mask words; a
 // first pass counts the set bits of every chunk, then one CTA per (chunk, pair) walks its words in
 // order: rank of a set pixel = set bits of the earlier chunks + block scan of the popcounts.
 // ------------------------------------------------------------------------------------------
@@ -76,19 +76,19 @@ __device__ __forceinline__ size_t motion_src(const int8_t* __restrict__ field, u
     return (size_t)yy * W + (uint32_t)xx;
 }
 
-// RS = 0: plain gather / scatter of the pixels; RS = 1 or 2: the gather stores residuals against J.prev per sample of RS bytes;
-// MC: against the motion-compensated J.prev (J.field, J.width) instead of the co-located pixel
+// RS = 0: plain gather of the pixels; RS = 1 or 2: residuals against J.prev per sample of RS bytes; MC: against the
+// motion-compensated J.prev (J.field, J.width) instead of the co-located pixel
 template <int PB, int RS, bool MC = false>
-__global__ void __launch_bounds__(1024) k_gather_scatter(const GatherJob* __restrict__ jobs, int scatter, uint32_t chunks,
-                                                          const uint32_t* __restrict__ counts, uint32_t* __restrict__ totals) {
+__global__ void __launch_bounds__(1024) k_gather(const GatherJob* __restrict__ jobs, uint32_t chunks, const uint32_t* __restrict__ counts) {
     static_assert(!MC || RS != 0, "motion gathers are residual gathers");
+    // set pixels before this chunk; summed before the job is loaded, so that the motion gathers fit 32 registers without spilling
+    uint32_t base = 0;
+    for (uint32_t i = 0; i < blockIdx.x; i++) base += counts[blockIdx.y * chunks + i];
     const GatherJob J = jobs[blockIdx.y];
     [[maybe_unused]] const uint32_t H = MC ? J.npix / J.width : 0u;
     __shared__ uint32_t s_warp[33];
     const uint32_t nwords = (J.npix + 31u) >> 5;
     const uint32_t w_begin = (uint32_t)(((uint64_t)nwords * blockIdx.x) / chunks), w_end = (uint32_t)(((uint64_t)nwords * (blockIdx.x + 1)) / chunks);
-    uint32_t base = 0;
-    for (uint32_t i = 0; i < blockIdx.x; i++) base += counts[blockIdx.y * chunks + i];   // set pixels before this chunk
     for (uint32_t w0 = w_begin; w0 < w_end; w0 += blockDim.x) {
         const uint32_t w = w0 + threadIdx.x;
         uint32_t m = (w < w_end) ? __ldg(J.mask + w) : 0u;
@@ -100,13 +100,11 @@ __global__ void __launch_bounds__(1024) k_gather_scatter(const GatherJob* __rest
             const size_t px = ((size_t)w << 5) + b;
             if constexpr (MC) resid_pixel<PB, RS>(J.values + (size_t)rank * PB, J.frame + px * PB, J.prev + motion_src(J.field, J.width, H, (uint32_t)px) * PB);
             else if constexpr (RS != 0) resid_pixel<PB, RS>(J.values + (size_t)rank * PB, J.frame + px * PB, J.prev + px * PB);
-            else if (scatter) copy_pixel<PB>(J.out_frame + px * PB, J.values + (size_t)rank * PB);
             else copy_pixel<PB>(J.values + (size_t)rank * PB, J.frame + px * PB);
             rank++;
         }
         base += tot;
     }
-    if (threadIdx.x == 0 && totals && blockIdx.x == chunks - 1) totals[blockIdx.y] = base;
 }
 
 // ------------------------------------------------------------------------------------------

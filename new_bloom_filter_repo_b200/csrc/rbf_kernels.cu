@@ -405,36 +405,35 @@ uint32_t gather_chunks(uint32_t npix) {
     if (ch > (uint32_t)GS_MAX_CHUNKS) ch = GS_MAX_CHUNKS;
     return ch < 1u ? 1u : ch;
 }
-// d_counts: F * gather_chunks(npix) uint32 of scratch; d_totals (may be NULL): set pixels per pair
-cudaError_t launch_gather_scatter(LaunchCfg& L, const GatherJob* d_jobs, int F, int scatter, uint32_t npix, uint32_t pix_bytes,
-                                  uint32_t* d_counts, uint32_t* d_totals, cudaStream_t st, uint32_t resid_sample_bytes, bool motion) {
+// d_counts: F * gather_chunks(npix) uint32 of scratch
+cudaError_t launch_gather(LaunchCfg& L, const GatherJob* d_jobs, int F, uint32_t npix, uint32_t pix_bytes, uint32_t* d_counts,
+                          cudaStream_t st, uint32_t resid_sample_bytes, bool motion) {
     if (F <= 0) return cudaSuccess;
     // the kernel is picked by (pixel bytes, residual sample bytes): 2 B per pixel is one 16-bit sample, never two 8-bit ones
     const uint32_t key = pix_bytes * 4u + resid_sample_bytes;
-    if ((resid_sample_bytes || motion) &&
-        (scatter || !(key == 1u * 4 + 1 || key == 3u * 4 + 1 || key == 2u * 4 + 2 || key == 6u * 4 + 2)))
+    if ((resid_sample_bytes || motion) && !(key == 1u * 4 + 1 || key == 3u * 4 + 1 || key == 2u * 4 + 2 || key == 6u * 4 + 2))
         return cudaErrorInvalidValue;                                 // checked before anything is launched
     const uint32_t ch = gather_chunks(npix);
     const dim3 grid(ch, (unsigned)F);
     k_mask_chunk_count<<<grid, 256, 0, st>>>(d_jobs, ch, d_counts);
     if (motion) {
         switch (key) {
-        case 1u * 4 + 1: k_gather_scatter<1, 1, true><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;
-        case 3u * 4 + 1: k_gather_scatter<3, 1, true><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;
-        case 2u * 4 + 2: k_gather_scatter<2, 2, true><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;
-        default: k_gather_scatter<6, 2, true><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;
+        case 1u * 4 + 1: k_gather<1, 1, true><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
+        case 3u * 4 + 1: k_gather<3, 1, true><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
+        case 2u * 4 + 2: k_gather<2, 2, true><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
+        default: k_gather<6, 2, true><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
         }
         return counted(L, 2);
     }
     switch (key) {
-    case 1u * 4: k_gather_scatter<1, 0><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
-    case 2u * 4: k_gather_scatter<2, 0><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
-    case 3u * 4: k_gather_scatter<3, 0><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
-    case 6u * 4: k_gather_scatter<6, 0><<<grid, 1024, 0, st>>>(d_jobs, scatter, ch, d_counts, d_totals); break;
-    case 1u * 4 + 1: k_gather_scatter<1, 1><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;   // 1 x 8 bit
-    case 3u * 4 + 1: k_gather_scatter<3, 1><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;   // 3 x 8 bit
-    case 2u * 4 + 2: k_gather_scatter<2, 2><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;   // 1 x 16 bit
-    case 6u * 4 + 2: k_gather_scatter<6, 2><<<grid, 1024, 0, st>>>(d_jobs, 0, ch, d_counts, d_totals); break;   // 3 x 16 bit
+    case 1u * 4: k_gather<1, 0><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
+    case 2u * 4: k_gather<2, 0><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
+    case 3u * 4: k_gather<3, 0><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
+    case 6u * 4: k_gather<6, 0><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
+    case 1u * 4 + 1: k_gather<1, 1><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;   // 1 x 8 bit
+    case 3u * 4 + 1: k_gather<3, 1><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;   // 3 x 8 bit
+    case 2u * 4 + 2: k_gather<2, 2><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;   // 1 x 16 bit
+    case 6u * 4 + 2: k_gather<6, 2><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;   // 3 x 16 bit
     default: return cudaErrorInvalidValue;
     }
     return counted(L, 2);
@@ -466,7 +465,7 @@ static cudaError_t launch_apply_sweep_t(LaunchCfg& L, const ApplyChain& A, cudaS
     k_apply_sweep<PB, RS><<<(A.ntiles + rounds - 1u) / rounds, AP_THREADS, 0, st>>>(A);
     return counted(L);
 }
-// (pixel bytes, residual sample bytes) as in launch_gather_scatter; 0: no residual pair, the plain sweep
+// (pixel bytes, residual sample bytes) as in launch_gather; 0: no residual pair, the plain sweep
 static bool apply_key_ok(uint32_t key) {
     return key == 1u * 4 || key == 2u * 4 || key == 3u * 4 || key == 6u * 4 || key == 1u * 4 + 1 || key == 3u * 4 + 1 ||
            key == 2u * 4 + 2 || key == 6u * 4 + 2;
@@ -494,7 +493,7 @@ cudaError_t launch_apply_chain(LaunchCfg& L, const ApplyChain& A, const uint8_t*
     auto mode = [&](uint32_t t) -> uint8_t { return h_modes ? h_modes[t] : 0; };
     bool any_residual = false, any_motion = false;
     for (uint32_t t = 0; t < A.count; t++) { any_residual |= mode(t) == 1; any_motion |= mode(t) == 2; }
-    const uint32_t mkey = A.pix_bytes * 4u + A.sample_bytes;           // the residual kinds of launch_gather_scatter
+    const uint32_t mkey = A.pix_bytes * 4u + A.sample_bytes;           // the residual kinds of launch_gather
     if (!apply_key_ok(A.pix_bytes * 4u + (any_residual ? A.sample_bytes : 0u)) || ((any_residual || any_motion) && !A.residual) ||
         (any_motion && (!d_fields || !apply_key_ok(mkey) || mkey == A.pix_bytes * 4u)))
         return cudaErrorInvalidValue;

@@ -38,10 +38,9 @@ struct PairJob {
 
 struct GatherJob {
     const uint32_t* mask;     // n bits, natural packing
-    const uint8_t* frame;     // gather: source (curr) frame; scatter: unused
+    const uint8_t* frame;     // source (curr) frame
     const uint8_t* prev;      // residual gather: the pair's previous frame (values = curr - prev per sample); otherwise unused
-    uint8_t* values;          // gather: output; scatter: input (rank-ordered pixel values)
-    uint8_t* out_frame;       // scatter: destination frame (already holds the base frame)
+    uint8_t* values;          // output (rank-ordered pixel values)
     uint32_t npix;
     uint32_t pix_bytes;
     uint32_t width;           // motion residual gather: frame width (the height is npix / width)
@@ -152,11 +151,10 @@ cudaError_t launch_witness(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t
 cudaError_t launch_expand(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t* d_scratch, uint32_t* d_consumed,
                           cudaStream_t st);
 uint32_t gather_chunks(uint32_t npix);
-// resid_sample_bytes: 0 gathers the current frame's samples; 1 or 2 gathers curr - prev per sample of that width (gather only,
-// pix_bytes / resid_sample_bytes channels of 1 or 3)
-cudaError_t launch_gather_scatter(LaunchCfg& L, const GatherJob* d_jobs, int F, int scatter, uint32_t npix, uint32_t pix_bytes,
-                                  uint32_t* d_counts, uint32_t* d_totals, cudaStream_t st, uint32_t resid_sample_bytes = 0,
-                                  bool motion = false);
+// resid_sample_bytes: 0 gathers the current frame's samples; 1 or 2 gathers curr - prev per sample of that width
+// (pix_bytes / resid_sample_bytes channels of 1 or 3)
+cudaError_t launch_gather(LaunchCfg& L, const GatherJob* d_jobs, int F, uint32_t npix, uint32_t pix_bytes, uint32_t* d_counts,
+                          cudaStream_t st, uint32_t resid_sample_bytes = 0, bool motion = false);
 // block motion search of F pairs (pairs[f].prev -> pairs[f].curr): d_fields + f * mv_blocks(H, W) * 2 receives the pair's vectors
 cudaError_t launch_motion_search(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t H, uint32_t W, uint32_t pix_bytes, uint32_t sample_bytes,
                                  int8_t* d_fields, cudaStream_t st);

@@ -265,7 +265,7 @@ class VideoFrameCompressor:
         return binary_diff, changed, density
 
     def _apply_frame_diff(self, base_frame, diff_mask: np.ndarray, changed_values: np.ndarray):   # ivc:849-909
-        """N2: the scatter runs on the device (k_gather_scatter); the result is a copy of base_frame's type.  Only mask entries
+        """N2: the apply runs on the device (the K4c sweep of one pair); the result is a copy of base_frame's type.  Only mask entries
         equal to 1 are applied (ivc:869).  Colour frames keep the base when the value count is not pixels x channels (ivc:882);
         grayscale frames, (h, w, 1) included, follow numpy's `frame[mask == 1] = values` (ivc:906-907): one value is broadcast,
         another count raises ValueError, and a mask without a set pixel leaves the frame as it is whatever the values.
@@ -283,7 +283,7 @@ class VideoFrameCompressor:
         if device:
             st = self._stream_for(data.shape, data.dtype, k1_only=True)
             st.upload(np.ascontiguousarray(data)[None], first=0)
-            st.apply_diff(0, 1, sel, vals)                     # value-count mismatch leaves the base unchanged (ivc:882)
+            st.apply_diff(0, sel, vals)                        # frame 1; a value-count mismatch leaves the base unchanged (ivc:882)
             data[...] = st.download(1).reshape(data.shape)
         elif color:                                            # ivc:872-903
             rows, cols = np.nonzero(sel)

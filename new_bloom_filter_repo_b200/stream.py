@@ -175,11 +175,11 @@ class FrameStream:
         _cabi.check(_cabi.lib().rbf_stream_motion_search(self._h, n, _cabi.ptr(out)), _cabi.ctx())
         return out
 
-    def apply_diff(self, base_frame: int, out_frame: int, mask: np.ndarray, values: np.ndarray) -> int:
-        """store[out_frame] = store[base_frame] with the pixels where `mask` is non-zero replaced by `values`, C samples of the
-        stream's dtype per pixel in row-major order; returns pixels applied.  When values does not hold exactly C samples per set
-        pixel, out_frame is a copy of base_frame and 0 is returned (ivc:882).  VideoFrameCompressor._apply_frame_diff passes
-        `mask == 1` (ivc:869)."""
+    def apply_diff(self, base_frame: int, mask: np.ndarray, values: np.ndarray) -> int:
+        """Frame (base_frame + 1) % max_frames = frame base_frame with the pixels where `mask` is non-zero replaced by `values`, C
+        samples of the stream's dtype per pixel in row-major order (apply_chain of one pair); returns pixels applied.  When values
+        does not hold exactly C samples per set pixel, that frame is a copy of base_frame and 0 is returned (ivc:882).
+        VideoFrameCompressor._apply_frame_diff passes `mask == 1` (ivc:869)."""
         m = np.asarray(mask)
         if m.size != self.npix:
             raise ValueError(f"a mask of {m.size} entries for frames of {self.npix} pixels")
@@ -189,15 +189,12 @@ class FrameStream:
         mk = np.packbits((m != 0).reshape(-1), bitorder="little")
         vals = np.ascontiguousarray(v).view(np.uint8).reshape(-1)
         applied = C.c_uint64()
-        _cabi.check(_cabi.lib().rbf_stream_apply_diff(self._h, int(base_frame), int(out_frame), _cabi.ptr(mk),
-                                                      _cabi.ptr(vals) if vals.size else None, vals.size, C.byref(applied)), _cabi.ctx())
+        _cabi.check(_cabi.lib().rbf_stream_apply_diff(self._h, int(base_frame), _cabi.ptr(mk), _cabi.ptr(vals) if vals.size else None,
+                                                      vals.size, C.byref(applied)), _cabi.ctx())
         return int(applied.value)
 
     def download(self, frame: int) -> np.ndarray:
-        shape = (self.H, self.W, self.C) if self.C > 1 else (self.H, self.W)
-        out = np.empty(shape, dtype=self.dtype)
-        _cabi.check(_cabi.lib().rbf_stream_download(self._h, int(frame), _cabi.ptr(out)), _cabi.ctx())
-        return out
+        return self.download_batch(frame, 1)[0]
 
     # ------------------------------------------------------------------ batched decode (K4b / K4c)
     def decode_masks(self, bitmaps: np.ndarray, witnesses: np.ndarray, l, wlen, k, raw, seeds=_cabi.IVC_SEEDS):

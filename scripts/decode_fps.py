@@ -22,7 +22,7 @@ from tests.util import synth_stream  # noqa: E402
 
 
 def per_frame_decode(comp, payloads):
-    """The per-frame route: keyframes one by one, each inter frame decoded, scattered and downloaded on its own."""
+    """The per-frame route: keyframes one by one, each inter frame decoded, applied and downloaded on its own."""
     frames, st = [], None
     for c in payloads:
         if not c.startswith((ivcmod._INTER_TAG, ivcmod._INTER_TAG_V1)):
@@ -42,7 +42,7 @@ def per_frame_decode(comp, payloads):
         if st is None:
             st = pkg.FrameStream(p.h, p.w, p.ch, dtype, max_frames=2, max_pairs=1, k1_only=True)
         st.upload(np.ascontiguousarray(prev.data if hasattr(prev, "yuv_info") else prev)[None], first=0)
-        assert st.apply_diff(0, 1, mask, values) == p.ones
+        assert st.apply_diff(0, mask, values) == p.ones
         out = st.download(1)
         frames.append(pkg.YUVFrame(out) if hasattr(prev, "yuv_info") else out)
     if st is not None:

@@ -277,7 +277,7 @@ def test_frame_diff_branches_and_thresholds(pkg, branch, dtype):
 
 
 def chunk_bounds(npix):
-    """Pixel index where each of the N1 gather's chunks after the first begins (rbf_kernels.cu: gather_chunks, k_gather_scatter)."""
+    """Pixel index where each of the N1 gather's chunks after the first begins (rbf_kernels.cu: gather_chunks, k_gather)."""
     nwords = (npix + 31) // 32
     ch = min(64, max(1, nwords // 4096))
     return [32 * (nwords * b // ch) for b in range(1, ch)]
@@ -397,40 +397,45 @@ def test_apply_frame_diff_hw1_with_hw_mask_follows_numpy(pkg):
 
 @pytest.mark.parametrize("dtype", [np.uint8, np.uint16])
 @pytest.mark.parametrize("channels", [1, 3])
-def test_stream_apply_diff_contract(pkg, dtype, channels):
-    """FrameStream.apply_diff, the layer under _apply_frame_diff: every non-zero mask entry is set (any dtype, 256 and 0.5 included);
-    values are C samples of the stream's dtype per set pixel or nothing is applied; a mask of another size or values of another dtype
-    raise before anything runs."""
+def test_stream_apply_diff_into_next_frame_contract(pkg, dtype, channels):
+    """FrameStream.apply_diff, the layer under _apply_frame_diff: frame base + 1 (modulo the store, the last slot included) is the
+    base with every non-zero mask entry set (any dtype, 256 and 0.5 included); values are C samples of the stream's dtype per set pixel
+    or the output is the base unchanged; a mask of another size or values of another dtype raise before anything runs.  The output
+    slot holds a third frame before each call, so a call that writes nothing fails."""
     rng = np.random.default_rng(channels + np.dtype(dtype).itemsize)
     hi = np.iinfo(dtype).max + 1
     shape = (19, 45) + ((channels,) if channels > 1 else ())
     base = rng.integers(0, hi, shape).astype(dtype)
+    other = base ^ dtype(1)                                                              # differs from base in every sample
     st = pkg.FrameStream(19, 45, channels, dtype, max_frames=3)
     try:
-        st.upload(base, first=0)
         for mdt, vals in ((bool, (0, 1)), (np.uint8, (0, 1, 2, 255)), (np.int16, (0, 1, 256, 257, -1)), (np.float64, (0.0, 1.0, 0.5, -2.0))):
             mask = rng.choice(np.array(vals, dtype=mdt), (19, 45))
             setp = mask != 0
             n = int(setp.sum())
             v = rng.integers(0, hi, n * channels).astype(dtype)
-            assert st.apply_diff(0, 2, mask, v) == n, mdt
             want = base.copy()
             want[setp] = v.reshape(-1, channels) if channels > 1 else v
-            assert np.array_equal(st.download(2), want), mdt
-            assert st.apply_diff(0, 1, mask, v[:-1]) == 0                                # one sample short: frame 1 = frame 0
-            assert np.array_equal(st.download(1), base)
+            for b, out in ((0, 1), (2, 0)):                                              # 2 -> 0: the slots wrap
+                st.upload(base, first=b)
+                st.upload(other, first=out)
+                assert st.apply_diff(b, mask, v) == n, (mdt, b)
+                assert np.array_equal(st.download(out), want), (mdt, b)
+                st.upload(other, first=out)
+                assert st.apply_diff(b, mask, v[:-1]) == 0, (mdt, b)                     # one sample short: the base
+                assert np.array_equal(st.download(out), base), (mdt, b)
         before = launches(pkg)
         with pytest.raises(ValueError):
-            st.apply_diff(0, 1, np.ones(19 * 45 - 1, np.uint8), np.zeros((19 * 45 - 1) * channels, dtype))
+            st.apply_diff(0, np.ones(19 * 45 - 1, np.uint8), np.zeros((19 * 45 - 1) * channels, dtype))
         with pytest.raises(ValueError):
-            st.apply_diff(0, 1, np.ones((19, 45), np.uint8), np.zeros(19 * 45 * channels, np.int64))
+            st.apply_diff(0, np.ones((19, 45), np.uint8), np.zeros(19 * 45 * channels, np.int64))
         assert launches(pkg) == before
     finally:
         st.close()
 
 
-def test_apply_happy_path_launches_only_the_scatter(pkg):
-    """_calculate_frame_diff + _apply_frame_diff of a grayscale and a colour pair: the apply costs the N2 count + scatter only."""
+def test_apply_happy_path_launches_only_the_chain_sweep(pkg):
+    """_calculate_frame_diff + _apply_frame_diff of a grayscale and a colour pair: the apply costs the one-pair K4c sweep only."""
     vfc = pkg.VideoFrameCompressor()
     for shape in ((64, 80), (64, 80, 3), (64, 80, 1)):
         prev, curr = frame_pair(shape, np.uint8, 3)
@@ -438,7 +443,7 @@ def test_apply_happy_path_launches_only_the_scatter(pkg):
         vfc._apply_frame_diff(prev, mask, vals)                                          # warm the cached stream
         before = launches(pkg)
         out = vfc._apply_frame_diff(prev, mask, vals)
-        assert launches(pkg) - before == 3, shape                                        # popcount, chunk count, scatter
+        assert launches(pkg) - before == 3, shape                                        # k_tile_count, k_tile_scan, k_apply_sweep
         assert np.array_equal(out, model_apply(prev, mask, vals))
 
 

@@ -455,7 +455,7 @@ def test_nccl_allgather_single_rank(pkg):
 # ------------------------------------------------------------------ SURVEY 8(f) N1 / N2 on the device
 @pytest.mark.parametrize("shape,dtype", [((64, 64), np.uint8), ((37, 53), np.uint8), ((270, 480), np.uint16), ((1080, 1920), np.uint8),
                                          ((2160, 3840), np.uint8), ((1080, 1920), np.uint16)])
-def test_gather_changed_and_apply_diff_vs_oracle(pkg, shape, dtype):
+def test_gather_changed_and_apply_diff_into_next_slot_vs_oracle(pkg, shape, dtype):
     from oracle import rbf_oracle as po
     frames = synth_stream(shape[0], shape[1], 4, 77, [0.05, 0.3, 0.0], dtype)
     st = pkg.FrameStream(shape[0], shape[1], 3, dtype, max_frames=6)
@@ -468,16 +468,19 @@ def test_gather_changed_and_apply_diff_vs_oracle(pkg, shape, dtype):
         expect = frames[t + 1][rows, cols, :].reshape(-1)                 # ivc:810-842, native sample type
         assert gathered[t].dtype == frames.dtype and np.array_equal(gathered[t], expect), t
         assert res[t].ones == len(rows)
-        # N2: rebuild frame t+1 from frame t on the device (slot 4 <- slot t)
-        applied = st.apply_diff(t, 4, mask, gathered[t])
-        assert applied == len(rows)
+        # N2: rebuild frame t+1 from frame t on the device (slot 5 <- slot 4, which holds frame t; slot 5 holds another frame)
         want = po.apply_frame_diff(frames[t], mask, expect)
-        assert np.array_equal(st.download(4), want)
+        st.upload(frames[t], first=4)
+        st.upload(want ^ dtype(1), first=5)
+        applied = st.apply_diff(4, mask, gathered[t])
+        assert applied == len(rows)
+        assert np.array_equal(st.download(5), want)
         assert np.array_equal(want, frames[t + 1])                        # every channel moves together in this stream
-    # value-count mismatch leaves the base frame unchanged (ivc:882)
+    # value-count mismatch leaves the base frame unchanged (ivc:882): slot 1 holds frame 1 before the call
     mask = po.frame_diff_mask(frames[0], frames[1], 3.0)
-    assert st.apply_diff(0, 5, mask, gathered[0][:-3]) == 0
-    assert np.array_equal(st.download(5), frames[0])
+    assert not np.array_equal(st.download(1), frames[0])
+    assert st.apply_diff(0, mask, gathered[0][:-3]) == 0
+    assert np.array_equal(st.download(1), frames[0])
     st.close()
 
 
