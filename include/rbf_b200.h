@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define RBF_ABI_VERSION 3
+#define RBF_ABI_VERSION 4
 
 typedef enum {
     RBF_OK = 0,
@@ -104,7 +104,6 @@ int rbf_malloc(rbf_ctx* ctx, size_t bytes, void** dptr);
 int rbf_free(rbf_ctx* ctx, void* dptr);
 int rbf_malloc_host(rbf_ctx* ctx, size_t bytes, void** hptr);   /* pinned */
 int rbf_free_host(rbf_ctx* ctx, void* hptr);
-int rbf_memcpy_h2d(rbf_ctx* ctx, void* dptr, const void* hptr, size_t bytes);
 int rbf_memcpy_d2h(rbf_ctx* ctx, void* hptr, const void* dptr, size_t bytes);
 int rbf_memset(rbf_ctx* ctx, void* dptr, int value, size_t bytes);
 
@@ -148,7 +147,7 @@ int rbf_stream_create(rbf_ctx* ctx, uint32_t height, uint32_t width, uint32_t ch
 void rbf_stream_destroy(rbf_stream* s);
 /* per-stream options (no process-global state: two compressors in one process do not interfere):
  *   "k1_only"   1: rbf_stream_encode stops after K1 (mask + counts) -- VideoFrameCompressor._calculate_frame_diff (ivc:784-808);
- *               infos report wlen = 0 and rbf_stream_fetch refuses bitmap / witness pointers
+ *               infos report wlen = 0 and rbf_stream_fetch_batch refuses bitmap / witness pointers
  *   "mask_mode" 0: |dY| > threshold (ivc:808); 1: additionally any byte of the pixel differs (lossless GOP mode)
  *   "gray_mode" 1: 3-channel frames are BGR and the mask is taken on cv2.cvtColor(.., COLOR_BGR2GRAY) (ivc:792-795),
  *               OpenCV's fixed point (3735 B + 19235 G + 9798 R + 16384) >> 15 for 8- and 16-bit samples
@@ -161,7 +160,6 @@ void rbf_stream_destroy(rbf_stream* s);
  *               likewise refused while motion_values is 1); a gather of more pairs than were searched fails too */
 int rbf_stream_set_option(rbf_stream* s, const char* key, int64_t value);
 int rbf_stream_upload(rbf_stream* s, uint32_t first_frame, uint32_t count, const void* host_frames);
-int rbf_stream_frame_ptr(rbf_stream* s, uint32_t frame, void** dptr);
 /* threshold: the Python float compared with `diff > threshold` (ivc:808).  k_override/l_override: NULL or [pairs]. */
 int rbf_stream_encode(rbf_stream* s, const uint32_t* prev_idx, const uint32_t* curr_idx, uint32_t pairs, double threshold,
                       const rbf_seeds* seeds, const double* k_override, const uint64_t* l_override, rbf_mask_info* infos_out);
@@ -169,12 +167,9 @@ int rbf_stream_encode(rbf_stream* s, const uint32_t* prev_idx, const uint32_t* c
 int rbf_stream_encode_host(rbf_stream* s, const void* host_frames, uint32_t nframes, double threshold, const rbf_seeds* seeds,
                            rbf_mask_info* infos_out, uint8_t* bitmaps_packbits_out, uint64_t bitmap_slot_bytes,
                            uint8_t* witness_packbits_out, uint64_t witness_slot_bytes);
-/* copy one pair's outputs to the host: bitmap/witness in packbits order (ceil(l/8), ceil(wlen/8) bytes),
- * mask as little-bit-order packed bytes (ceil(n/8)); any pointer may be NULL */
-int rbf_stream_fetch(rbf_stream* s, uint32_t pair, uint8_t* bitmap_packbits, uint8_t* witness_packbits,
-                     uint8_t* mask_packed_little);
-/* the same for pairs [first, first+count) at once: output k of a kind lands at base + k*slot_bytes (slot_bytes bytes are copied
- * per pair, capped at the device slot); one synchronisation for the whole batch.  NULL pointers are skipped. */
+/* copy the outputs of pairs [first, first+count) to the host: bitmap/witness in packbits order (a pair's ceil(l/8), ceil(wlen/8)
+ * bytes), mask as little-bit-order packed bytes (ceil(n/8)); output k of a kind lands at base + k*slot_bytes (slot_bytes bytes are
+ * copied per pair, capped at the device slot); one synchronisation for the whole batch.  NULL pointers are skipped. */
 int rbf_stream_fetch_batch(rbf_stream* s, uint32_t first, uint32_t count, uint8_t* bitmaps_packbits, uint64_t bitmap_slot_bytes,
                            uint8_t* witness_packbits, uint64_t witness_slot_bytes, uint8_t* masks_packed_little,
                            uint64_t mask_slot_bytes);
@@ -251,7 +246,6 @@ int rbf_stream_download_batch(rbf_stream* s, uint32_t first, uint32_t count, voi
 /* N3  the 5x5 median of cv2.medianBlur in VideoFrameCompressor._estimate_noise_level (ivc:738): replicated border, 13th
  *     smallest of 25, exact for uint8 / uint16.  The float32 std of (frame - median) stays in numpy (ivc:741-744). */
 int rbf_median_blur5(rbf_ctx* ctx, const void* plane_in, uint32_t height, uint32_t width, uint32_t sample_bytes, void* plane_out);
-int rbf_stream_median5(rbf_stream* s, uint32_t frame, void* plane_out);   /* channel 0 of a resident frame */
 
 /* ---- SURVEY 8(f) row N4: the zlib entropy stage (fvc:31, ivc:956) coded on the device.  Each input buffer becomes one zlib
  *     stream (RFC 1950/1951) that zlib.decompress reads; the bytes differ from zlib's own, the decoded data do not.  Layout:
@@ -301,7 +295,6 @@ int rbf_stream_inflate_values(rbf_stream* s, uint32_t count, const void* const* 
  * over NVLink.  NCCL is dlopen'ed (libnccl.so.2); the unique id travels over the caller's own channel. */
 int rbf_nccl_unique_id(uint8_t id_out[128]);
 int rbf_nccl_init(rbf_ctx* ctx, const uint8_t id[128], int rank, int nranks);
-int rbf_nccl_allgather(rbf_ctx* ctx, const void* d_send, void* d_recv, uint64_t bytes_per_rank);
 /* compact `pairs` bitmap slots (slot_bytes each) into d_send and all-gather them into d_recv.  Enqueued on the context's
  * communication stream so that the next rbf_stream_encode overlaps the exchange; d_recv is complete after rbf_sync,
  * rbf_timer_stop_ms or rbf_memcpy_d2h. */

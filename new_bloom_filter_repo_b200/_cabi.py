@@ -32,7 +32,7 @@ class MaskInfo(C.Structure):
                 ("floor_k", C.c_uint32), ("raw", C.c_uint32)]
 
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 IVC_SEEDS = (0x12345678, 0x87654321, 999)    # improved_video_compressor.py:62-63,94
 BC_SEEDS = (0, 1, 999)                       # bloom_compress.py:163-164,195
 
@@ -42,17 +42,17 @@ EXPORTS = [
     "rbf_timer_start", "rbf_timer_stop_ms",
     "rbf_xxh64", "rbf_hash_decimal", "rbf_hash_decimal_century", "rbf_probe_index",
     "rbf_activation_threshold", "rbf_optimal_params",
-    "rbf_malloc", "rbf_free", "rbf_malloc_host", "rbf_free_host", "rbf_memcpy_h2d", "rbf_memcpy_d2h", "rbf_memset",
+    "rbf_malloc", "rbf_free", "rbf_malloc_host", "rbf_free_host", "rbf_memcpy_d2h", "rbf_memset",
     "rbf_filter_create", "rbf_filter_destroy", "rbf_filter_add_indices", "rbf_filter_check_indices",
     "rbf_filter_add_strings", "rbf_filter_check_strings", "rbf_filter_get_bits", "rbf_filter_set_bits",
     "rbf_compress_mask", "rbf_decompress_mask",
-    "rbf_stream_create", "rbf_stream_destroy", "rbf_stream_set_option", "rbf_stream_upload", "rbf_stream_frame_ptr", "rbf_stream_encode",
-    "rbf_stream_encode_host", "rbf_stream_fetch", "rbf_stream_fetch_batch", "rbf_stream_decode_verify", "rbf_stream_bitmap_region", "rbf_stream_stage_ms",
-    "rbf_stream_gather_changed", "rbf_stream_apply_diff", "rbf_median_blur5", "rbf_stream_median5",
+    "rbf_stream_create", "rbf_stream_destroy", "rbf_stream_set_option", "rbf_stream_upload", "rbf_stream_encode",
+    "rbf_stream_encode_host", "rbf_stream_fetch_batch", "rbf_stream_decode_verify", "rbf_stream_bitmap_region", "rbf_stream_stage_ms",
+    "rbf_stream_gather_changed", "rbf_stream_apply_diff", "rbf_median_blur5",
     "rbf_stream_decode_masks", "rbf_stream_apply_chain", "rbf_stream_motion_search", "rbf_stream_download_batch",
     "rbf_zlib_bound", "rbf_deflate_code_lengths", "rbf_zlib_compress_batch", "rbf_stream_zlib_changed",
     "rbf_inflate_segment", "rbf_zlib_decompress_batch", "rbf_stream_inflate_values",
-    "rbf_nccl_unique_id", "rbf_nccl_init", "rbf_nccl_allgather", "rbf_stream_allgather_bitmaps", "rbf_nccl_destroy",
+    "rbf_nccl_unique_id", "rbf_nccl_init", "rbf_stream_allgather_bitmaps", "rbf_nccl_destroy",
     "rbf_peer_export", "rbf_peer_open", "rbf_peer_close", "rbf_peer_gather_init", "rbf_peer_gather_half", "rbf_peer_gather_shutdown",
 ]
 
@@ -90,7 +90,6 @@ def _sig(L):
     L.rbf_free.argtypes = [vp, vp]
     L.rbf_malloc_host.argtypes = [vp, C.c_size_t, P(vp)]
     L.rbf_free_host.argtypes = [vp, vp]
-    L.rbf_memcpy_h2d.argtypes = [vp, vp, vp, C.c_size_t]
     L.rbf_memcpy_d2h.argtypes = [vp, vp, vp, C.c_size_t]
     L.rbf_memset.argtypes = [vp, vp, i32, C.c_size_t]
     L.rbf_filter_create.argtypes = [vp, u64, dbl, P(Seeds), P(vp)]
@@ -109,10 +108,8 @@ def _sig(L):
     L.rbf_stream_destroy.restype = None
     L.rbf_stream_set_option.argtypes = [vp, C.c_char_p, C.c_int64]
     L.rbf_stream_upload.argtypes = [vp, u32, u32, vp]
-    L.rbf_stream_frame_ptr.argtypes = [vp, u32, P(vp)]
     L.rbf_stream_encode.argtypes = [vp, vp, vp, u32, dbl, P(Seeds), vp, vp, vp]
     L.rbf_stream_encode_host.argtypes = [vp, vp, u32, dbl, P(Seeds), vp, vp, u64, vp, u64]
-    L.rbf_stream_fetch.argtypes = [vp, u32, vp, vp, vp]
     L.rbf_stream_fetch_batch.argtypes = [vp, u32, u32, vp, u64, vp, u64, vp, u64]
     L.rbf_stream_decode_verify.argtypes = [vp, u32, vp]
     L.rbf_stream_bitmap_region.argtypes = [vp, P(vp), P(u64)]
@@ -124,7 +121,6 @@ def _sig(L):
     L.rbf_stream_motion_search.argtypes = [vp, u32, vp]
     L.rbf_stream_download_batch.argtypes = [vp, u32, u32, vp]
     L.rbf_median_blur5.argtypes = [vp, vp, u32, u32, u32, vp]
-    L.rbf_stream_median5.argtypes = [vp, u32, vp]
     L.rbf_zlib_bound.argtypes = [u64]
     L.rbf_zlib_bound.restype = u64
     L.rbf_deflate_code_lengths.argtypes = [vp, u32, u32, vp]
@@ -135,7 +131,6 @@ def _sig(L):
     L.rbf_stream_inflate_values.argtypes = [vp, u32, vp, vp, vp, vp, vp]
     L.rbf_nccl_unique_id.argtypes = [vp]
     L.rbf_nccl_init.argtypes = [vp, vp, i32, i32]
-    L.rbf_nccl_allgather.argtypes = [vp, vp, vp, u64]
     L.rbf_stream_allgather_bitmaps.argtypes = [vp, u32, u64, vp, vp]
     L.rbf_nccl_destroy.argtypes = [vp]
     L.rbf_peer_export.argtypes = [vp, vp, vp]

@@ -336,10 +336,6 @@ extern "C" int rbf_malloc(rbf_ctx* c, size_t bytes, void** d) { if (!c || !d) re
 extern "C" int rbf_free(rbf_ctx* c, void* d) { if (!c) return RBF_ERR_INVALID; if (d) CK(c, cudaFree(d)); return RBF_OK; }
 extern "C" int rbf_malloc_host(rbf_ctx* c, size_t bytes, void** h) { if (!c || !h) return RBF_ERR_INVALID; CK(c, cudaMallocHost(h, bytes ? bytes : 1)); return RBF_OK; }
 extern "C" int rbf_free_host(rbf_ctx* c, void* h) { if (!c) return RBF_ERR_INVALID; if (h) CK(c, cudaFreeHost(h)); return RBF_OK; }
-extern "C" int rbf_memcpy_h2d(rbf_ctx* c, void* d, const void* h, size_t n) {
-    if (!c) return RBF_ERR_INVALID;
-    CK(c, cudaMemcpyAsync(d, h, n, cudaMemcpyHostToDevice, c->st)); CK(c, cudaStreamSynchronize(c->st)); c->h2d += n; return RBF_OK;
-}
 extern "C" int rbf_memcpy_d2h(rbf_ctx* c, void* h, const void* d, size_t n) {
     if (!c) return RBF_ERR_INVALID;
     if (int r = join_comm(c)) return r;
@@ -727,11 +723,6 @@ extern "C" int rbf_stream_upload(rbf_stream* s, uint32_t first, uint32_t count, 
     CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
 }
-extern "C" int rbf_stream_frame_ptr(rbf_stream* s, uint32_t frame, void** dptr) {
-    if (!s || !dptr || frame >= s->max_frames) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_frame_ptr: bad argument");
-    *dptr = s->d_frames + (size_t)frame * s->frame_stride;
-    return RBF_OK;
-}
 extern "C" int rbf_stream_bitmap_region(rbf_stream* s, void** dptr, uint64_t* stride) {
     if (!s) return RBF_ERR_INVALID;
     if (dptr) *dptr = s->d_bits;
@@ -1041,20 +1032,6 @@ extern "C" int rbf_stream_stage_ms(rbf_stream* s, double out[6]) {
     CK(c, span(3, 4, &out[3]));     // K3
     CK(c, span(4, 5, &out[4]));     // K3b (pass count, witness, packbits order)
     CK(c, span(0, 5, &out[5]));     // whole encode
-    return RBF_OK;
-}
-
-extern "C" int rbf_stream_fetch(rbf_stream* s, uint32_t pair, uint8_t* bitmap, uint8_t* witness, uint8_t* mask_little) {
-    if (!s) return RBF_ERR_INVALID;
-    rbf_ctx* c = s->c;
-    if (pair >= s->last_pairs) return set_err(c, RBF_ERR_INVALID, "pair %u was not encoded", pair);
-    if (s->last_k1_only && (bitmap || witness))
-        return set_err(c, RBF_ERR_STATE, "the last encode stopped after K1 (k1_only): there is no bitmap / witness to fetch");
-    const rbf_mask_info& in = s->last_infos[pair];
-    if (bitmap && !in.raw) { size_t nb = (in.l + 7) / 8; CK(c, cudaMemcpyAsync(bitmap, s->d_bits + (size_t)pair * s->mask_stride_w, nb, cudaMemcpyDeviceToHost, c->st)); c->d2h += nb; }
-    if (witness && !in.raw && in.wlen) { size_t nb = (in.wlen + 7) / 8; CK(c, cudaMemcpyAsync(witness, s->d_wit + (size_t)pair * s->mask_stride_w, nb, cudaMemcpyDeviceToHost, c->st)); c->d2h += nb; }
-    if (mask_little) { size_t nb = (s->npix + 7) / 8; CK(c, cudaMemcpyAsync(mask_little, s->d_mask + (size_t)pair * s->mask_stride_w, nb, cudaMemcpyDeviceToHost, c->st)); c->d2h += nb; }
-    CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
 }
 
@@ -1469,21 +1446,7 @@ extern "C" int rbf_median_blur5(rbf_ctx* c, const void* plane_in, uint32_t H, ui
     int rc;
     if ((rc = scratch_get(c, kScrMedianIn, bytes, &d_in)) || (rc = scratch_get(c, kScrMedianOut, bytes, &d_out))) return rc;
     CK(c, cudaMemcpyAsync(d_in, plane_in, bytes, cudaMemcpyHostToDevice, c->st)); c->h2d += (int64_t)bytes;
-    CK(c, launch_median5(c->L, d_in, 1, H, W, (int)sample_bytes, d_out, c->st));
-    CK(c, cudaMemcpyAsync(plane_out, d_out, bytes, cudaMemcpyDeviceToHost, c->st)); c->d2h += (int64_t)bytes;
-    CK(c, cudaStreamSynchronize(c->st));
-    return RBF_OK;
-}
-
-extern "C" int rbf_stream_median5(rbf_stream* s, uint32_t frame, void* plane_out) {
-    if (!s || !plane_out || frame >= s->max_frames) return set_err(s ? s->c : nullptr, RBF_ERR_INVALID, "rbf_stream_median5: bad argument");
-    rbf_ctx* c = s->c;
-    CK(c, cudaSetDevice(c->device));
-    const size_t bytes = (size_t)s->npix * s->S;
-    void* d_out;
-    int rc;
-    if ((rc = scratch_get(c, kScrMedianOut, bytes, &d_out))) return rc;
-    CK(c, launch_median5(c->L, s->d_frames + (size_t)frame * s->frame_stride, s->C, s->H, s->W, (int)s->S, d_out, c->st));
+    CK(c, launch_median5(c->L, d_in, H, W, (int)sample_bytes, d_out, c->st));
     CK(c, cudaMemcpyAsync(plane_out, d_out, bytes, cudaMemcpyDeviceToHost, c->st)); c->d2h += (int64_t)bytes;
     CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
@@ -1870,8 +1833,8 @@ extern "C" int rbf_nccl_init(rbf_ctx* c, const uint8_t id[128], int rank, int nr
     c->nccl_lib = h; c->nccl_comm = comm; c->rank = rank; c->nranks = nranks;
     return RBF_OK;
 }
+// The caller has checked that c->nccl_comm is initialised.
 static int nccl_allgather_on(rbf_ctx* c, const void* d_send, void* d_recv, uint64_t bytes_per_rank, cudaStream_t st) {
-    if (!c || !c->nccl_comm) return set_err(c, RBF_ERR_STATE, "rbf_nccl_allgather: communicator not initialised");
     fn_AllGather f = (fn_AllGather)dlsym(c->nccl_lib, "ncclAllGather");
     if (!f) return set_err(c, RBF_ERR_NCCL, "ncclAllGather not found");
     int r = f(d_send, d_recv, (size_t)bytes_per_rank, /*ncclUint8*/ 1, c->nccl_comm, st);
@@ -1881,9 +1844,6 @@ static int nccl_allgather_on(rbf_ctx* c, const void* d_send, void* d_recv, uint6
     }
     c->L.launches++;
     return RBF_OK;
-}
-extern "C" int rbf_nccl_allgather(rbf_ctx* c, const void* d_send, void* d_recv, uint64_t bytes_per_rank) {
-    return nccl_allgather_on(c, d_send, d_recv, bytes_per_rank, c ? c->st : nullptr);
 }
 // Packs the bit arrays of the last encode into fixed-size slots and all-gathers them on the context's communication
 // stream: the call returns once the work is enqueued, the next rbf_stream_encode overlaps it (it only waits for the

@@ -109,13 +109,12 @@ __global__ void __launch_bounds__(1024) k_gather(const GatherJob* __restrict__ j
 
 // ------------------------------------------------------------------------------------------
 // N3 (SURVEY 8f): the 5x5 median of cv2.medianBlur (ivc:738) -- replicated border, 13th smallest of
-// the 25 samples -- on channel 0 of an interleaved frame.  Rank selection (25 x 25 comparisons) is
+// the 25 samples -- of one plane.  Rank selection (25 x 25 comparisons) is
 // exact for any sample type; the float32 std that follows (ivc:741-744) stays in numpy on the host so
 // that the noise estimate is bit-identical to the reference's.
 // ------------------------------------------------------------------------------------------
 template <typename T>
-__global__ void __launch_bounds__(256) k_median5(const T* __restrict__ in, uint32_t pix_stride, uint32_t H, uint32_t W,
-                                                  T* __restrict__ out) {
+__global__ void __launch_bounds__(256) k_median5(const T* __restrict__ in, uint32_t H, uint32_t W, T* __restrict__ out) {
     const uint32_t x = blockIdx.x * 32u + (threadIdx.x & 31u), y = blockIdx.y * 8u + (threadIdx.x >> 5);
     if (x >= W || y >= H) return;
     uint32_t v[25];
@@ -125,7 +124,7 @@ __global__ void __launch_bounds__(256) k_median5(const T* __restrict__ in, uint3
 #pragma unroll
         for (int dx = -2; dx <= 2; dx++) {
             const uint32_t xx = (uint32_t)min(max((int)x + dx, 0), (int)W - 1);
-            v[(dy + 2) * 5 + (dx + 2)] = (uint32_t)__ldg(in + ((size_t)yy * W + xx) * pix_stride);
+            v[(dy + 2) * 5 + (dx + 2)] = (uint32_t)__ldg(in + (size_t)yy * W + xx);
         }
     }
     uint32_t med = 0;

@@ -542,12 +542,11 @@ cudaError_t launch_motion_search(LaunchCfg& L, const PairJob* d_pairs, int F, ui
     }
     return counted(L);
 }
-cudaError_t launch_median5(LaunchCfg& L, const void* d_in, uint32_t pix_stride, uint32_t H, uint32_t W, int sample_bytes, void* d_out,
-                           cudaStream_t st) {
+cudaError_t launch_median5(LaunchCfg& L, const void* d_in, uint32_t H, uint32_t W, int sample_bytes, void* d_out, cudaStream_t st) {
     if (H == 0 || W == 0) return cudaSuccess;
     dim3 grid((W + 31u) / 32u, (H + 7u) / 8u);
-    if (sample_bytes == 1) k_median5<uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)d_in, pix_stride, H, W, (uint8_t*)d_out);
-    else if (sample_bytes == 2) k_median5<uint16_t><<<grid, 256, 0, st>>>((const uint16_t*)d_in, pix_stride, H, W, (uint16_t*)d_out);
+    if (sample_bytes == 1) k_median5<uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)d_in, H, W, (uint8_t*)d_out);
+    else if (sample_bytes == 2) k_median5<uint16_t><<<grid, 256, 0, st>>>((const uint16_t*)d_in, H, W, (uint16_t*)d_out);
     else return cudaErrorInvalidValue;
     return counted(L);
 }

@@ -171,8 +171,7 @@ cudaError_t launch_mask_popcount(LaunchCfg& L, const uint32_t* d_masks, size_t s
 // from the run's start), read only after a motion pair.
 cudaError_t launch_apply_chain(LaunchCfg& L, const ApplyChain& A, const uint8_t* h_modes, const int8_t* d_fields, uint32_t H,
                                uint32_t W, uint32_t* d_run_bad, cudaStream_t st);
-cudaError_t launch_median5(LaunchCfg& L, const void* d_in, uint32_t pix_stride, uint32_t H, uint32_t W, int sample_bytes, void* d_out,
-                           cudaStream_t st);
+cudaError_t launch_median5(LaunchCfg& L, const void* d_in, uint32_t H, uint32_t W, int sample_bytes, void* d_out, cudaStream_t st);
 cudaError_t launch_bitrev(LaunchCfg& L, uint32_t* d_words, size_t nwords, cudaStream_t st);
 cudaError_t launch_unpack_bits(LaunchCfg& L, const uint32_t* d_words, uint8_t* d_out, size_t nbits, cudaStream_t st);
 cudaError_t launch_unpack_bits_msb(LaunchCfg& L, const uint32_t* d_words, uint8_t* d_out, size_t nbits, cudaStream_t st);

@@ -107,9 +107,11 @@ class FrameStream:
             bm = np.zeros((int(mi.l) + 7) // 8, dtype=np.uint8)
             wt = np.zeros((int(mi.wlen) + 7) // 8, dtype=np.uint8)
         mk = np.zeros((self.npix + 7) // 8, dtype=np.uint8) if want_mask else None
-        _cabi.check(_cabi.lib().rbf_stream_fetch(self._h, int(pair), _cabi.ptr(bm) if bm.size else None,
-                                                 _cabi.ptr(wt) if wt.size else None,
-                                                 _cabi.ptr(mk) if mk is not None else None), _cabi.ctx())
+        args = []                                          # one-pair slots of exactly each output's bytes; NULL, 0 for what is not copied
+        for a, coded in ((bm, not mi.raw), (wt, not mi.raw), (mk, True)):
+            copy = a is not None and a.size > 0 and coded
+            args += [_cabi.ptr(a) if copy else None, a.size if copy else 0]
+        _cabi.check(_cabi.lib().rbf_stream_fetch_batch(self._h, int(pair), 1, *args), _cabi.ctx())
         mask = np.unpackbits(mk, bitorder="little")[: self.npix] if mk is not None else None
         return bm, wt, mask
 

@@ -28,7 +28,7 @@ def test_header_symbols_exported(cabi):
     missing = [n for n in declared if not hasattr(L, n)]
     assert not missing, missing
     assert sorted(cabi.EXPORTS) == declared
-    assert cabi.lib().rbf_abi_version() == 3
+    assert cabi.lib().rbf_abi_version() == 4
 
 
 def test_host_xxh64_matches_golden(cabi):

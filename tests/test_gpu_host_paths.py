@@ -33,33 +33,48 @@ def _set(pkg, **opts):
 DEFAULTS = dict(encode_ranges=1, kq_ranges=1, host_chunk_frames=32)
 
 
-def profiled_kernels(fn):
-    """Runs fn() under torch.profiler with CUDA activities -> (fn's result, [(kernel name, grid, block)] of the library's kernels in
-    start order).  Memcpy and memset activities are not kernels and are left out.  A torch kernel opens the window, synchronised
-    before fn runs: the trace has been seen to lose the first kernels of a window."""
+def counted_run(pkg, fn, name, counts):
+    """fn() inside the range "entry <name>" of the open profiler session -> fn's result; counts[name] = its kernel_launches delta."""
     import torch
-    from torch.profiler import ProfilerActivity, profile
+    L, ctx = pkg._cabi.lib(), pkg._cabi.ctx()
     torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        torch.ones(1, device="cuda").add_(1)
-        torch.cuda.synchronize()
+    before = L.rbf_get_counter(ctx, b"kernel_launches")
+    with torch.profiler.record_function("entry " + name):
         out = fn()
         torch.cuda.synchronize()
+    counts[name] = L.rbf_get_counter(ctx, b"kernel_launches") - before
+    return out
+
+
+def profiled_kernels(run):
+    """run(counts) under ONE torch.profiler session with CPU and CUDA activities -> {name: (counts[name], [(kernel name, grid, block)]
+    of the library's kernels launched inside the range "entry <name>", in start order)}.  A kernel belongs to the range that holds
+    its launch call (the trace links the two by correlation id).  Memcpy and memset activities are not kernels and are left out.
+    One session, opened by a synchronised torch kernel: in a process that had already run other tests, a trace of one short session
+    per entry point lost kernels, sometimes a whole session's."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    counts = {}
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        torch.ones(1, device="cuda").add_(1)
+        torch.cuda.synchronize()
+        run(counts)
     with tempfile.TemporaryDirectory() as d:
         path = os.path.join(d, "trace.json")
         prof.export_chrome_trace(path)
         with open(path) as f:
             events = json.load(f)["traceEvents"]
+    ranges = {e["name"][len("entry "):]: (e["ts"], e["ts"] + e["dur"]) for e in events
+              if e.get("cat") == "user_annotation" and e["name"].startswith("entry ")}
+    assert sorted(ranges) == sorted(counts), (sorted(ranges), sorted(counts))
+    launched = {e["args"]["correlation"]: e["ts"] for e in events if e.get("cat") == "cuda_runtime" and "correlation" in e.get("args", {})}
     ks = sorted((e for e in events if e.get("cat") == "kernel" and "rbf::" in e["name"]), key=lambda e: e["ts"])
-    return out, [(e["name"], tuple(e["args"].get("grid", ())), tuple(e["args"].get("block", ()))) for e in ks]
-
-
-def counted_run(pkg, fn):
-    """-> (fn's result, kernel_launches delta, kernels the profiler recorded)."""
-    L, ctx = pkg._cabi.lib(), pkg._cabi.ctx()
-    before = L.rbf_get_counter(ctx, b"kernel_launches")
-    out, ks = profiled_kernels(fn)
-    return out, L.rbf_get_counter(ctx, b"kernel_launches") - before, ks
+    out = {}
+    for name, (t0, t1) in ranges.items():
+        mine = [e for e in ks if t0 <= launched.get(e["args"].get("correlation"), -1) <= t1]
+        out[name] = (counts[name], [(e["name"], tuple(e["args"].get("grid", ())), tuple(e["args"].get("block", ()))) for e in mine])
+    return out
 
 
 def _decode_inputs(st, res, n):
@@ -76,56 +91,46 @@ def _decode_inputs(st, res, n):
     return (bitmaps, wt, [r.l for r in res], [r.wlen for r in res], [r.k for r in res], [int(r.raw) for r in res])
 
 
-def entry_points(pkg, h, w):
-    """Every host path under test -> {name: (kernel_launches delta, profiled kernels)}."""
+def entry_points(pkg, h, w, counts):
+    """Every host path under test, each through counted_run."""
     frames = synth_stream(h, w, NFR, 11, P_SEQ)
-    out = {}
     st = pkg.FrameStream(h, w, 3, np.uint8, max_frames=NFR, max_pairs=NFR - 1)
     try:
         for name, opts in (("encode", {}), ("encode_ranges4", dict(encode_ranges=4)), ("encode_kq4", dict(kq_ranges=4))):
             st.upload(frames)
             _set(pkg, **dict(DEFAULTS, **opts))
             try:
-                res, n, ks = counted_run(pkg, lambda: st.encode_consecutive(NFR, THR))
+                res = counted_run(pkg, lambda: st.encode_consecutive(NFR, THR), name, counts)
             finally:
                 _set(pkg, **DEFAULTS)
-            out[name] = (n, ks)
         assert any(r.raw for r in res) and not all(r.raw for r in res)
         _set(pkg, host_chunk_frames=3)
         try:
-            res, n, ks = counted_run(pkg, lambda: st.encode_host(frames, THR))
+            res = counted_run(pkg, lambda: st.encode_host(frames, THR), "encode_host", counts)
         finally:
             _set(pkg, **DEFAULTS)
-        out["encode_host"] = (n, ks)
-        mism, n, ks = counted_run(pkg, st.decode_verify)
+        mism = counted_run(pkg, st.decode_verify, "decode_verify", counts)
         assert not mism.any()
-        out["decode_verify"] = (n, ks)
-        vals, n, ks = counted_run(pkg, st.gather_changed)
-        out["gather_changed"] = (n, ks)
-        zs, n, ks = counted_run(pkg, st.zlib_changed)
-        out["zlib_changed"] = (n, ks)
+        vals = counted_run(pkg, st.gather_changed, "gather_changed", counts)
+        counted_run(pkg, st.zlib_changed, "zlib_changed", counts)
         args = _decode_inputs(st, res, h * w)
-        _, n, ks = counted_run(pkg, lambda: (st.decode_masks(*args), st.apply_chain(0, vals)))
-        out["decode_masks+apply_chain"] = (n, ks)
+        counted_run(pkg, lambda: (st.decode_masks(*args), st.apply_chain(0, vals)), "decode_masks+apply_chain", counts)
         assert np.array_equal(st.download(NFR - 1), frames[-1])
     finally:
         _set(pkg, **DEFAULTS)
         st.close()
     mask = (frames[1] != frames[0]).any(-1).reshape(-1).astype(np.uint8)
     bfc = pkg.BloomFilterCompressor()
-    (bm, wt, _, n_, _), n, ks = counted_run(pkg, lambda: bfc.compress(mask))
-    out["compress"] = (n, ks)
-    dec, n, ks = counted_run(pkg, lambda: bfc.decompress(bm, wt, n_, bfc.last_info.k))
+    bm, wt, _, n_, _ = counted_run(pkg, lambda: bfc.compress(mask), "compress", counts)
+    dec = counted_run(pkg, lambda: bfc.decompress(bm, wt, n_, bfc.last_info.k), "decompress", counts)
     assert np.array_equal(dec, mask)
-    out["decompress"] = (n, ks)
-    return out
 
 
 @gpu
 @pytest.mark.parametrize("h,w", [(120, 160), (1080, 1920)])
 def test_launch_counter_equals_kernels_run(pkg, h, w):
     """120x160 has one witness chunk (K3b and K4b skip the pass-count kernel); 1080p has several."""
-    for name, (n, ks) in entry_points(pkg, h, w).items():
+    for name, (n, ks) in profiled_kernels(lambda counts: entry_points(pkg, h, w, counts)).items():
         assert ks, (name, "the profiler recorded no kernel")
         assert n == len(ks), (name, n, [k[0][:60] for k in ks])
 
