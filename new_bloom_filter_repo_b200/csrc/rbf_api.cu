@@ -697,8 +697,6 @@ extern "C" int rbf_stream_set_option(rbf_stream* s, const char* key, int64_t v) 
     }
     if (!strcmp(key, "value_mode")) {
         if (v != 0 && v != 1) return set_err(s->c, RBF_ERR_INVALID, "value_mode must be 0 (values) or 1 (residuals), not %lld", (long long)v);
-        if (v && !((s->C == 1 || s->C == 3) && (s->S == 1 || s->S == 2)))
-            return set_err(s->c, RBF_ERR_INVALID, "residual values need 1 or 3 channels of 8- or 16-bit samples (C=%u S=%u)", s->C, s->S);
         if (v && s->motion_values) return set_err(s->c, RBF_ERR_INVALID, "value_mode 1 and motion_values 1 exclude each other");
         s->value_mode = (int)v;
         return RBF_OK;
@@ -1187,8 +1185,8 @@ static int gather_values(rbf_stream* s, uint32_t pairs, const uint64_t* offs, ui
         J.field = s->motion_values ? s->d_fields + i * field_bytes : nullptr;
     }
     CK(c, cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(GatherJob) * pairs, cudaMemcpyHostToDevice, c->st));   // pageable: staged before return
-    CK(c, launch_gather(c->L, (const GatherJob*)d_jobs, (int)pairs, (uint32_t)s->npix, pb, (uint32_t*)d_gcnt, c->st,
-                        s->value_mode || s->motion_values ? s->S : 0u, s->motion_values != 0));
+    CK(c, launch_gather(c->L, (const GatherJob*)d_jobs, (int)pairs, (uint32_t)s->npix, pb, s->S, s->motion_values ? 2 : s->value_mode,
+                        (uint32_t*)d_gcnt, c->st));
     *d_values = (uint8_t*)d_vals;
     return RBF_OK;
 }

@@ -22,6 +22,7 @@
 #include <stdint.h>
 
 #include <mutex>
+#include <type_traits>
 
 #include "rbf_kernels.cuh"
 
@@ -127,6 +128,17 @@ static cudaError_t counted(LaunchCfg& L, int kernels = 1) {
     return cudaGetLastError();
 }
 
+// The four frame formats a stream can have (1 or 3 channels of 1- or 2-byte samples, fixed by rbf_stream_create) as compile-time
+// (pixel bytes, sample bytes): f(ic<PB>, ic<S>) launches that format's kernel instances.  Any other format launches nothing.
+template <int N> using ic = std::integral_constant<int, N>;
+template <class F> static cudaError_t by_format(uint32_t pix_bytes, uint32_t sample_bytes, F&& f) {
+    if (pix_bytes == 1 && sample_bytes == 1) return f(ic<1>{}, ic<1>{});
+    if (pix_bytes == 3 && sample_bytes == 1) return f(ic<3>{}, ic<1>{});
+    if (pix_bytes == 2 && sample_bytes == 2) return f(ic<2>{}, ic<2>{});
+    if (pix_bytes == 6 && sample_bytes == 2) return f(ic<6>{}, ic<2>{});
+    return cudaErrorInvalidValue;
+}
+
 // K1 over a chain of F >= 2 pairs: persistent sweeps, each of the same number of tiles (or one fewer).
 // sms == 0: the whole GPU, one sweep per CTA and at most ctas_per_sm CTAs per SM.
 // sms > 0: one wide CTA on each of `sms` SMs, with as many sweeps as fit in its shared memory (SW_MAX_SWEEPS at most).  Its
@@ -205,19 +217,13 @@ static cudaError_t launch_threshold_t(LaunchCfg& L, const PairJob* d_pairs, int 
 cudaError_t launch_threshold(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t npix, int channels, int sample_bytes, int thr_int,
                              int any_mode, int gray_mode, uint32_t* d_ones, uint32_t* d_resid, bool chain, int sms, cudaStream_t st) {
     if (F <= 0 || npix == 0) return cudaSuccess;
-    const int pb = channels * sample_bytes, cap = L.k1_ctas_per_sm;
-#define RBF_K1(PB_, S_, GRAY_) launch_threshold_t<PB_, S_, GRAY_>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, sms, st)
-    if (gray_mode) {
-        if (pb == 3 && sample_bytes == 1) return RBF_K1(3, 1, true);
-        if (pb == 6 && sample_bytes == 2) return RBF_K1(6, 2, true);
-        return cudaErrorInvalidValue;
-    }
-    if (pb == 3 && sample_bytes == 1) return RBF_K1(3, 1, false);
-    if (pb == 6 && sample_bytes == 2) return RBF_K1(6, 2, false);
-    if (pb == 1 && sample_bytes == 1) return RBF_K1(1, 1, false);
-    if (pb == 2 && sample_bytes == 2) return RBF_K1(2, 2, false);
-#undef RBF_K1
-    return cudaErrorInvalidValue;
+    return by_format((uint32_t)(channels * sample_bytes), (uint32_t)sample_bytes, [&](auto PBc, auto Sc) -> cudaError_t {
+        constexpr int PB = decltype(PBc)::value, S = decltype(Sc)::value;
+        const int cap = L.k1_ctas_per_sm;
+        if (!gray_mode) return launch_threshold_t<PB, S, false>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, sms, st);
+        if constexpr (PB == 3 * S) return launch_threshold_t<PB, S, true>(L, d_pairs, F, npix, thr_int, any_mode, d_ones, d_resid, chain, cap, sms, st);
+        else return cudaErrorInvalidValue;                        // gray needs three channels
+    });
 }
 
 static cudaLaunchConfig_t insert_cluster_config(uint32_t cs, uint32_t units, cudaStream_t st, cudaLaunchAttribute* attr) {
@@ -406,37 +412,19 @@ uint32_t gather_chunks(uint32_t npix) {
     return ch < 1u ? 1u : ch;
 }
 // d_counts: F * gather_chunks(npix) uint32 of scratch
-cudaError_t launch_gather(LaunchCfg& L, const GatherJob* d_jobs, int F, uint32_t npix, uint32_t pix_bytes, uint32_t* d_counts,
-                          cudaStream_t st, uint32_t resid_sample_bytes, bool motion) {
+cudaError_t launch_gather(LaunchCfg& L, const GatherJob* d_jobs, int F, uint32_t npix, uint32_t pix_bytes, uint32_t sample_bytes,
+                          int kind, uint32_t* d_counts, cudaStream_t st) {
     if (F <= 0) return cudaSuccess;
-    // the kernel is picked by (pixel bytes, residual sample bytes): 2 B per pixel is one 16-bit sample, never two 8-bit ones
-    const uint32_t key = pix_bytes * 4u + resid_sample_bytes;
-    if ((resid_sample_bytes || motion) && !(key == 1u * 4 + 1 || key == 3u * 4 + 1 || key == 2u * 4 + 2 || key == 6u * 4 + 2))
-        return cudaErrorInvalidValue;                                 // checked before anything is launched
-    const uint32_t ch = gather_chunks(npix);
-    const dim3 grid(ch, (unsigned)F);
-    k_mask_chunk_count<<<grid, 256, 0, st>>>(d_jobs, ch, d_counts);
-    if (motion) {
-        switch (key) {
-        case 1u * 4 + 1: k_gather<1, 1, true><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
-        case 3u * 4 + 1: k_gather<3, 1, true><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
-        case 2u * 4 + 2: k_gather<2, 2, true><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
-        default: k_gather<6, 2, true><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
-        }
+    return by_format(pix_bytes, sample_bytes, [&](auto PBc, auto Sc) -> cudaError_t {
+        constexpr int PB = decltype(PBc)::value, S = decltype(Sc)::value;
+        const uint32_t ch = gather_chunks(npix);
+        const dim3 grid(ch, (unsigned)F);
+        k_mask_chunk_count<<<grid, 256, 0, st>>>(d_jobs, ch, d_counts);
+        if (kind == 0) k_gather<PB, 0, false><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts);
+        else if (kind == 1) k_gather<PB, S, false><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts);
+        else k_gather<PB, S, true><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts);
         return counted(L, 2);
-    }
-    switch (key) {
-    case 1u * 4: k_gather<1, 0><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
-    case 2u * 4: k_gather<2, 0><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
-    case 3u * 4: k_gather<3, 0><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
-    case 6u * 4: k_gather<6, 0><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;
-    case 1u * 4 + 1: k_gather<1, 1><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;   // 1 x 8 bit
-    case 3u * 4 + 1: k_gather<3, 1><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;   // 3 x 8 bit
-    case 2u * 4 + 2: k_gather<2, 2><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;   // 1 x 16 bit
-    case 6u * 4 + 2: k_gather<6, 2><<<grid, 1024, 0, st>>>(d_jobs, ch, d_counts); break;   // 3 x 16 bit
-    default: return cudaErrorInvalidValue;
-    }
-    return counted(L, 2);
+    });
 }
 cudaError_t launch_raw_masks(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t npix, cudaStream_t st) {
     if (F <= 0 || npix == 0) return cudaSuccess;
@@ -465,23 +453,6 @@ static cudaError_t launch_apply_sweep_t(LaunchCfg& L, const ApplyChain& A, cudaS
     k_apply_sweep<PB, RS><<<(A.ntiles + rounds - 1u) / rounds, AP_THREADS, 0, st>>>(A);
     return counted(L);
 }
-// (pixel bytes, residual sample bytes) as in launch_gather; 0: no residual pair, the plain sweep
-static bool apply_key_ok(uint32_t key) {
-    return key == 1u * 4 || key == 2u * 4 || key == 3u * 4 || key == 6u * 4 || key == 1u * 4 + 1 || key == 3u * 4 + 1 ||
-           key == 2u * 4 + 2 || key == 6u * 4 + 2;
-}
-static cudaError_t launch_sweep(LaunchCfg& L, const ApplyChain& A, uint32_t key, cudaStream_t st) {
-    switch (key) {
-    case 1u * 4: return launch_apply_sweep_t<1, 0>(L, A, st);
-    case 2u * 4: return launch_apply_sweep_t<2, 0>(L, A, st);
-    case 3u * 4: return launch_apply_sweep_t<3, 0>(L, A, st);
-    case 6u * 4: return launch_apply_sweep_t<6, 0>(L, A, st);
-    case 1u * 4 + 1: return launch_apply_sweep_t<1, 1>(L, A, st);
-    case 3u * 4 + 1: return launch_apply_sweep_t<3, 1>(L, A, st);
-    case 2u * 4 + 2: return launch_apply_sweep_t<2, 2>(L, A, st);
-    default: return launch_apply_sweep_t<6, 2>(L, A, st);
-    }
-}
 static void launch_tile_prefix(LaunchCfg& L, const ApplyChain& A, cudaStream_t st) {
     k_tile_count<<<dim3((A.ntiles + 7u) / 8u, A.count), 256, 0, st>>>(A);
     k_tile_scan<<<A.count, 1024, 0, st>>>(A);
@@ -490,57 +461,46 @@ static void launch_tile_prefix(LaunchCfg& L, const ApplyChain& A, cudaStream_t s
 cudaError_t launch_apply_chain(LaunchCfg& L, const ApplyChain& A, const uint8_t* h_modes, const int8_t* d_fields, uint32_t H,
                                uint32_t W, uint32_t* d_run_bad, cudaStream_t st) {
     if (A.count == 0 || A.ntiles == 0) return cudaSuccess;
-    auto mode = [&](uint32_t t) -> uint8_t { return h_modes ? h_modes[t] : 0; };
-    bool any_residual = false, any_motion = false;
-    for (uint32_t t = 0; t < A.count; t++) { any_residual |= mode(t) == 1; any_motion |= mode(t) == 2; }
-    const uint32_t mkey = A.pix_bytes * 4u + A.sample_bytes;           // the residual kinds of launch_gather
-    if (!apply_key_ok(A.pix_bytes * 4u + (any_residual ? A.sample_bytes : 0u)) || ((any_residual || any_motion) && !A.residual) ||
-        (any_motion && (!d_fields || !apply_key_ok(mkey) || mkey == A.pix_bytes * 4u)))
-        return cudaErrorInvalidValue;
-    launch_tile_prefix(L, A, st);
-    for (uint32_t t = 0; t < A.count;) {
-        if (mode(t) == 2) {
-            uint32_t* next_bad = t + 1u < A.count && mode(t + 1u) != 2 ? d_run_bad + t + 1u : nullptr;
-            switch (mkey) {
-            case 1u * 4 + 1: k_apply_motion<1, 1><<<A.ntiles, AP_THREADS, 0, st>>>(A, t, d_fields, H, W, next_bad); break;
-            case 3u * 4 + 1: k_apply_motion<3, 1><<<A.ntiles, AP_THREADS, 0, st>>>(A, t, d_fields, H, W, next_bad); break;
-            case 2u * 4 + 2: k_apply_motion<2, 2><<<A.ntiles, AP_THREADS, 0, st>>>(A, t, d_fields, H, W, next_bad); break;
-            default: k_apply_motion<6, 2><<<A.ntiles, AP_THREADS, 0, st>>>(A, t, d_fields, H, W, next_bad); break;
+    return by_format(A.pix_bytes, A.sample_bytes, [&](auto PBc, auto Sc) -> cudaError_t {
+        constexpr int PB = decltype(PBc)::value, S = decltype(Sc)::value;
+        auto mode = [&](uint32_t t) -> uint8_t { return h_modes ? h_modes[t] : 0; };
+        launch_tile_prefix(L, A, st);
+        for (uint32_t t = 0; t < A.count;) {
+            if (mode(t) == 2) {
+                uint32_t* next_bad = t + 1u < A.count && mode(t + 1u) != 2 ? d_run_bad + t + 1u : nullptr;
+                k_apply_motion<PB, S><<<A.ntiles, AP_THREADS, 0, st>>>(A, t, d_fields, H, W, next_bad);
+                if (cudaError_t e = counted(L)) return e;
+                t++;
+                continue;
             }
-            if (cudaError_t e = counted(L)) return e;
-            t++;
-            continue;
+            // a run of plain / residual pairs [t, t1) is swept as a chain of its own (without a motion pair: the whole chain, A as
+            // given); a run after a motion pair checks the first failing pair counted from its start, which that motion kernel stored
+            uint32_t t1 = t;
+            bool run_residual = false;
+            for (; t1 < A.count && mode(t1) != 2; t1++) run_residual |= mode(t1) != 0;
+            ApplyChain R = A;
+            R.masks = A.masks + (size_t)t * A.mask_stride_w;
+            R.base = A.base + t >= A.max_frames ? A.base + t - A.max_frames : A.base + t;
+            R.count = t1 - t;
+            R.value_off = A.value_off + t;
+            R.residual = run_residual ? A.residual + t : nullptr;
+            R.tile_pfx = A.tile_pfx + (size_t)t * A.ntiles;
+            R.first_bad = t == 0 ? A.first_bad : d_run_bad + t;
+            const cudaError_t e = run_residual ? launch_apply_sweep_t<PB, S>(L, R, st) : launch_apply_sweep_t<PB, 0>(L, R, st);
+            if (e != cudaSuccess) return e;
+            t = t1;
         }
-        // a run of plain / residual pairs [t, t1) is swept as a chain of its own (without a motion pair: the whole chain, A as
-        // given); a run after a motion pair checks the first failing pair counted from its start, which that motion kernel stored
-        uint32_t t1 = t;
-        bool run_residual = false;
-        for (; t1 < A.count && mode(t1) != 2; t1++) run_residual |= mode(t1) != 0;
-        ApplyChain R = A;
-        R.masks = A.masks + (size_t)t * A.mask_stride_w;
-        R.base = A.base + t >= A.max_frames ? A.base + t - A.max_frames : A.base + t;
-        R.count = t1 - t;
-        R.value_off = A.value_off + t;
-        R.residual = run_residual ? A.residual + t : nullptr;
-        R.tile_pfx = A.tile_pfx + (size_t)t * A.ntiles;
-        R.first_bad = t == 0 ? A.first_bad : d_run_bad + t;
-        if (cudaError_t e = launch_sweep(L, R, A.pix_bytes * 4u + (run_residual ? A.sample_bytes : 0u), st)) return e;
-        t = t1;
-    }
-    return cudaSuccess;
+        return cudaSuccess;
+    });
 }
 cudaError_t launch_motion_search(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t H, uint32_t W, uint32_t pix_bytes, uint32_t sample_bytes,
                                  int8_t* d_fields, cudaStream_t st) {
     if (F <= 0 || H == 0 || W == 0) return cudaSuccess;
-    const dim3 grid(mv_blocks(H, W), (unsigned)F);
-    switch (pix_bytes * 4u + sample_bytes) {
-    case 1u * 4 + 1: k_motion_search<1, 1><<<grid, MV_THREADS, 0, st>>>(d_pairs, H, W, d_fields); break;
-    case 3u * 4 + 1: k_motion_search<3, 1><<<grid, MV_THREADS, 0, st>>>(d_pairs, H, W, d_fields); break;
-    case 2u * 4 + 2: k_motion_search<2, 2><<<grid, MV_THREADS, 0, st>>>(d_pairs, H, W, d_fields); break;
-    case 6u * 4 + 2: k_motion_search<6, 2><<<grid, MV_THREADS, 0, st>>>(d_pairs, H, W, d_fields); break;
-    default: return cudaErrorInvalidValue;
-    }
-    return counted(L);
+    return by_format(pix_bytes, sample_bytes, [&](auto PBc, auto Sc) -> cudaError_t {
+        constexpr int PB = decltype(PBc)::value, S = decltype(Sc)::value;
+        k_motion_search<PB, S><<<dim3(mv_blocks(H, W), (unsigned)F), MV_THREADS, 0, st>>>(d_pairs, H, W, d_fields);
+        return counted(L);
+    });
 }
 cudaError_t launch_median5(LaunchCfg& L, const void* d_in, uint32_t H, uint32_t W, int sample_bytes, void* d_out, cudaStream_t st) {
     if (H == 0 || W == 0) return cudaSuccess;

@@ -151,10 +151,10 @@ cudaError_t launch_witness(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t
 cudaError_t launch_expand(LaunchCfg& L, const FrameJob* d_jobs, int F, uint32_t max_centuries, uint32_t* d_scratch, uint32_t* d_consumed,
                           cudaStream_t st);
 uint32_t gather_chunks(uint32_t npix);
-// resid_sample_bytes: 0 gathers the current frame's samples; 1 or 2 gathers curr - prev per sample of that width
-// (pix_bytes / resid_sample_bytes channels of 1 or 3)
-cudaError_t launch_gather(LaunchCfg& L, const GatherJob* d_jobs, int F, uint32_t npix, uint32_t pix_bytes, uint32_t* d_counts,
-                          cudaStream_t st, uint32_t resid_sample_bytes = 0, bool motion = false);
+// kind, as the per-pair modes of K4c: 0 gathers the current frame's samples; 1 curr - prev per sample of sample_bytes; 2 curr minus
+// the motion-compensated prev.  A format other than a stream's (pix_bytes, sample_bytes) launches nothing (cudaErrorInvalidValue).
+cudaError_t launch_gather(LaunchCfg& L, const GatherJob* d_jobs, int F, uint32_t npix, uint32_t pix_bytes, uint32_t sample_bytes,
+                          int kind, uint32_t* d_counts, cudaStream_t st);
 // block motion search of F pairs (pairs[f].prev -> pairs[f].curr): d_fields + f * mv_blocks(H, W) * 2 receives the pair's vectors
 cudaError_t launch_motion_search(LaunchCfg& L, const PairJob* d_pairs, int F, uint32_t H, uint32_t W, uint32_t pix_bytes, uint32_t sample_bytes,
                                  int8_t* d_fields, cudaStream_t st);
