@@ -78,7 +78,7 @@ int rbf_device_info(rbf_ctx* ctx, char* name, int name_len, int* sm_count, int* 
  * "pipe_k1_sms" (the SMs its K1 runs on beside K2), "k1_ctas_per_sm" (K1 grid cap); "k1_only" / "mask_mode" here are only the defaults that
  * streams created afterwards inherit -- per-stream state lives in rbf_stream_set_option. */
 int rbf_set_option(rbf_ctx* ctx, const char* key, int64_t value);
-int64_t rbf_get_counter(rbf_ctx* ctx, const char* key);   /* "kernel_launches", "h2d_bytes", "d2h_bytes" */
+int64_t rbf_get_counter(rbf_ctx* ctx, const char* key);   /* "kernel_launches", "h2d_bytes", "d2h_bytes", "d2d_bytes" */
 int rbf_reset_counters(rbf_ctx* ctx);
 int rbf_sync(rbf_ctx* ctx);
 /* device-side timing on the context's stream (CUDA events) */
@@ -243,6 +243,13 @@ int rbf_stream_apply_chain(rbf_stream* s, uint32_t base_frame, uint32_t count, c
  * stay in the stream for the motion_values gathers until the next encode or rbf_stream_decode_masks.  One synchronisation. */
 int rbf_stream_motion_search(rbf_stream* s, uint32_t pairs, int8_t* fields_out);
 int rbf_stream_download_batch(rbf_stream* s, uint32_t first, uint32_t count, void* host_out);
+/* frames first .. first+count-1 (slots modulo max_frames) into a contiguous device buffer (count x frame_bytes), device to
+ * device.  wait_stream: 0, or a cudaStream_t of the caller whose pending work must finish before dst is written
+ * (1 = cudaStreamLegacy, 2 = cudaStreamPerThread, as in __cuda_array_interface__ v3).  Returns after the copy has completed.
+ * RBF_ERR_INVALID, with nothing enqueued, for first >= max_frames, count 0 or > max_frames, a NULL dst, dst_capacity below
+ * count x frame_bytes, or a dst that is not device or managed memory of the context's device.  Counted as "d2d_bytes". */
+int rbf_stream_copy_frames(rbf_stream* s, uint32_t first, uint32_t count, void* dst_device, uint64_t dst_capacity,
+                           uint64_t wait_stream);
 /* N3  the 5x5 median of cv2.medianBlur in VideoFrameCompressor._estimate_noise_level (ivc:738): replicated border, 13th
  *     smallest of 25, exact for uint8 / uint16.  The float32 std of (frame - median) stays in numpy (ivc:741-744). */
 int rbf_median_blur5(rbf_ctx* ctx, const void* plane_in, uint32_t height, uint32_t width, uint32_t sample_bytes, void* plane_out);

@@ -10,12 +10,12 @@ There is no CPU fallback: importing is cheap, but every entry point needs librbf
 from . import _cabi
 from . import deflate
 from ._cabi import RbfError
-from .improved_video_compressor import (BloomFilterCompressor, ImprovedVideoCompressor, VideoFrameCompressor)
+from .improved_video_compressor import (BloomFilterCompressor, ImprovedVideoCompressor, VideoFrameCompressor, VideoReader)
 from .improved_video_compressor import RationalBloomFilter as IndexRationalBloomFilter
 from .rational_bloom_filter import RationalBloomFilter, StandardBloomFilter
 from .fixed_video_compressor import FixedVideoCompressor, YUVFrame
 from .stream import FrameStream, PairResult
 
-__all__ = ["ImprovedVideoCompressor", "VideoFrameCompressor", "BloomFilterCompressor", "IndexRationalBloomFilter",
+__all__ = ["ImprovedVideoCompressor", "VideoReader", "VideoFrameCompressor", "BloomFilterCompressor", "IndexRationalBloomFilter",
            "RationalBloomFilter", "StandardBloomFilter", "FixedVideoCompressor", "YUVFrame", "FrameStream",
            "PairResult", "RbfError", "deflate"]

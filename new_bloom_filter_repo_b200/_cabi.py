@@ -50,7 +50,7 @@ EXPORTS = [
     "rbf_stream_encode_host", "rbf_stream_fetch_batch", "rbf_stream_decode_verify", "rbf_stream_bitmap_region", "rbf_stream_stage_ms",
     "rbf_stream_gather_changed", "rbf_stream_apply_diff", "rbf_median_blur5",
     "rbf_stream_decode_masks", "rbf_stream_apply_chain", "rbf_stream_motion_search", "rbf_stream_download_batch",
-    "rbf_zlib_bound", "rbf_deflate_code_lengths", "rbf_zlib_compress_batch", "rbf_stream_zlib_changed",
+    "rbf_stream_copy_frames", "rbf_zlib_bound", "rbf_deflate_code_lengths", "rbf_zlib_compress_batch", "rbf_stream_zlib_changed",
     "rbf_inflate_segment", "rbf_zlib_decompress_batch", "rbf_stream_inflate_values",
     "rbf_nccl_unique_id", "rbf_nccl_init", "rbf_stream_allgather_bitmaps", "rbf_nccl_destroy",
     "rbf_peer_export", "rbf_peer_open", "rbf_peer_close", "rbf_peer_gather_init", "rbf_peer_gather_half", "rbf_peer_gather_shutdown",
@@ -120,6 +120,7 @@ def _sig(L):
     L.rbf_stream_apply_chain.argtypes = [vp, u32, u32, vp, vp, vp, vp, vp]
     L.rbf_stream_motion_search.argtypes = [vp, u32, vp]
     L.rbf_stream_download_batch.argtypes = [vp, u32, u32, vp]
+    L.rbf_stream_copy_frames.argtypes = [vp, u32, u32, vp, u64, u64]
     L.rbf_median_blur5.argtypes = [vp, vp, u32, u32, u32, vp]
     L.rbf_zlib_bound.argtypes = [u64]
     L.rbf_zlib_bound.restype = u64

@@ -51,7 +51,8 @@ struct rbf_ctx {
     int mask_mode = 0;      // 0: |dY| > thr (ivc:808); 1: additionally any byte of the pixel differs
     int kq_ranges = 1;      // > 1: K2 of range r+1 runs beside K3 of range r (see stream_encode_pipelined)
     char err[512];
-    int64_t h2d = 0, d2h = 0;
+    int64_t h2d = 0, d2h = 0, d2d = 0;   // d2d: rbf_stream_copy_frames into caller device memory
+    cudaEvent_t ev_wait = nullptr;        // rbf_stream_copy_frames: the caller's stream, recorded before the copy
     std::vector<void*> scratch;
     std::vector<size_t> scratch_sz;
     // NCCL (dlopen'ed)
@@ -237,6 +238,7 @@ extern "C" void rbf_ctx_destroy(rbf_ctx* c) {
     for (void* p : c->scratch) if (p) cudaFree(p);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
+    if (c->ev_wait) cudaEventDestroy(c->ev_wait);
     if (c->st) cudaStreamDestroy(c->st);
     if (c->st_k1) cudaStreamDestroy(c->st_k1);
     if (c->st_d2h) cudaStreamDestroy(c->st_d2h);
@@ -288,9 +290,10 @@ extern "C" int64_t rbf_get_counter(rbf_ctx* c, const char* key) {
     if (!strcmp(key, "kernel_launches")) return c->L.launches;
     if (!strcmp(key, "h2d_bytes")) return c->h2d;
     if (!strcmp(key, "d2h_bytes")) return c->d2h;
+    if (!strcmp(key, "d2d_bytes")) return c->d2d;
     return -1;
 }
-extern "C" int rbf_reset_counters(rbf_ctx* c) { if (!c) return RBF_ERR_INVALID; c->L.launches = c->h2d = c->d2h = 0; return RBF_OK; }
+extern "C" int rbf_reset_counters(rbf_ctx* c) { if (!c) return RBF_ERR_INVALID; c->L.launches = c->h2d = c->d2h = c->d2d = 0; return RBF_OK; }
 // before the bit arrays are overwritten: the slot packing of a pending all-gather must have read them
 static int wait_pack(rbf_ctx* c) {
     if (c->pack_pending) { CK(c, cudaStreamWaitEvent(c->st, c->ev_pack, 0)); c->pack_pending = false; }
@@ -1427,6 +1430,41 @@ extern "C" int rbf_stream_download_batch(rbf_stream* s, uint32_t first, uint32_t
         CK(c, cudaMemcpy2DAsync((uint8_t*)host_out + (size_t)head * s->frame_bytes, s->frame_bytes, s->d_frames, s->frame_stride,
                                 s->frame_bytes, count - head, cudaMemcpyDeviceToHost, c->st));
     c->d2h += (int64_t)s->frame_bytes * count;
+    CK(c, cudaStreamSynchronize(c->st));
+    return RBF_OK;
+}
+
+// rbf_stream_download_batch into device memory: the caller's pending work on wait_stream (its __cuda_array_interface__ stream) is
+// ordered before the copy through an event, so a buffer still being written or read there is not overwritten early.
+extern "C" int rbf_stream_copy_frames(rbf_stream* s, uint32_t first, uint32_t count, void* dst_device, uint64_t dst_capacity,
+                                      uint64_t wait_stream) {
+    if (!s) return set_err(nullptr, RBF_ERR_INVALID, "rbf_stream_copy_frames: stream is NULL");
+    rbf_ctx* c = s->c;
+    if (first >= s->max_frames || count == 0 || count > s->max_frames)
+        return set_err(c, RBF_ERR_INVALID, "rbf_stream_copy_frames: frames %u + %u of a store of %u", first, count, s->max_frames);
+    const uint64_t bytes = s->frame_bytes * count;
+    if (!dst_device || dst_capacity < bytes)
+        return set_err(c, RBF_ERR_INVALID, "rbf_stream_copy_frames: %llu bytes into a buffer of %llu", (unsigned long long)bytes,
+                       dst_device ? (unsigned long long)dst_capacity : 0ULL);
+    CK(c, cudaSetDevice(c->device));
+    cudaPointerAttributes pa;
+    cudaError_t e = cudaPointerGetAttributes(&pa, dst_device);
+    if (e != cudaSuccess) cudaGetLastError();                    // not a pointer the runtime knows: refused below
+    if (e != cudaSuccess || !(pa.type == cudaMemoryTypeDevice || pa.type == cudaMemoryTypeManaged) || pa.device != c->device)
+        return set_err(c, RBF_ERR_INVALID, "rbf_stream_copy_frames: dst is not device or managed memory of device %d", c->device);
+    if (wait_stream) {
+        cudaStream_t ws = wait_stream == 1 ? cudaStreamLegacy : wait_stream == 2 ? cudaStreamPerThread : (cudaStream_t)(uintptr_t)wait_stream;
+        if (!c->ev_wait) CK(c, cudaEventCreateWithFlags(&c->ev_wait, cudaEventDisableTiming));
+        CK(c, cudaEventRecord(c->ev_wait, ws));
+        CK(c, cudaStreamWaitEvent(c->st, c->ev_wait, 0));
+    }
+    const uint32_t head = count < s->max_frames - first ? count : s->max_frames - first;   // slots wrap as in rbf_stream_apply_chain
+    CK(c, cudaMemcpy2DAsync(dst_device, s->frame_bytes, s->d_frames + (size_t)first * s->frame_stride, s->frame_stride, s->frame_bytes,
+                            head, cudaMemcpyDeviceToDevice, c->st));
+    if (head < count)
+        CK(c, cudaMemcpy2DAsync((uint8_t*)dst_device + (size_t)head * s->frame_bytes, s->frame_bytes, s->d_frames, s->frame_stride,
+                                s->frame_bytes, count - head, cudaMemcpyDeviceToDevice, c->st));
+    c->d2d += (int64_t)bytes;
     CK(c, cudaStreamSynchronize(c->st));
     return RBF_OK;
 }

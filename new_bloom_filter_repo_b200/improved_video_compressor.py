@@ -19,9 +19,11 @@ keyframe / inter-frame loop the reference's `keyframe_interval` argument promise
 """
 from __future__ import annotations
 
+import bisect
 import ctypes as C
 import io
 import math
+import operator
 import os
 import struct
 import time
@@ -394,6 +396,83 @@ class _InterJob:
         self.l = self.wlen = self.vsize = 0
 
 
+def _is_inter(payload) -> bool:
+    """Whether a payload is an inter frame (its first 8 bytes are an inter tag) rather than a keyframe."""
+    return bytes(payload[:len(_INTER_TAG)]) in _INTER_TAGS
+
+
+class _Jobs:
+    """The decode jobs of a file's payloads (ImprovedVideoCompressor._start_inter / _start_key), started in file order from
+    payload(i), for payloads before `stop` only.  take(i) hands job i over, starting it and the `ahead` payloads after it first if
+    they have not been, and forgets it, so a decode holds only the payloads of the jobs it is working on and of those started ahead."""
+
+    def __init__(self, comp: "ImprovedVideoCompressor", payload, inter: List[bool], pool, stop: int, ahead: int = 0):
+        self._comp, self._payload, self._inter, self._pool, self._stop, self._ahead = comp, payload, inter, pool, stop, ahead
+        self._jobs: Dict[int, object] = {}
+        self._next = 0
+
+    def start(self, upto: int, first: int = 0) -> None:
+        """Starts the jobs of payloads [max(first, next), upto) (`first`: where the decode begins; earlier payloads are never read)."""
+        self._next = max(self._next, first)
+        for i in range(self._next, min(upto, self._stop)):
+            c = self._payload(i)
+            self._jobs[i] = self._comp._start_inter(c, self._pool) if self._inter[i] else self._comp._start_key(c, self._pool)
+            self._next = i + 1
+
+    def take(self, i: int):
+        self.start(i + 1 + self._ahead, i)
+        return self._jobs.pop(i)
+
+
+class _DeviceOut:
+    """A caller's device buffer, any object with __cuda_array_interface__, that file frames start .. stop-1 are written to with
+    FrameStream.copy_frames.  The shape must be (stop - start, H, W) for one channel or (stop - start, H, W, C) for more, the dtype
+    uint8 or uint16, the layout C-contiguous.  The interface's stream (v3) is waited for before each copy; an interface without
+    one (v2, as torch exports) is ordered after the legacy default stream, where torch's default stream runs."""
+
+    def __init__(self, out, start: int, stop: int):
+        cai = getattr(out, "__cuda_array_interface__", None)
+        if not isinstance(cai, dict):
+            raise ValueError("out must be device memory with __cuda_array_interface__")
+        shape, dtype = tuple(int(x) for x in cai["shape"]), np.dtype(cai["typestr"])
+        if len(shape) not in (3, 4) or shape[0] != stop - start or (len(shape) == 4 and shape[3] < 2):
+            raise ValueError(f"out has shape {shape}, not ({stop - start}, H, W) or ({stop - start}, H, W, C) with C > 1")
+        if dtype not in (np.dtype(np.uint8), np.dtype(np.uint16)):
+            raise ValueError(f"out has dtype {dtype}; frames are uint8 or uint16")
+        strides = cai.get("strides")                         # None: C-contiguous
+        if strides is not None and any(n > 1 and s != dtype.itemsize * math.prod(shape[d + 1:])
+                                       for d, (n, s) in enumerate(zip(shape, strides))):
+            raise ValueError("out must be C-contiguous")
+        ptr, readonly = cai["data"]
+        if readonly:
+            raise ValueError("out is read-only")
+        self.ptr, self.start, self.stop, self.dtype = int(ptr), start, stop, dtype
+        self.frame_shape = shape[1:] if len(shape) == 4 else shape[1:3]
+        self.frame_bytes = math.prod(self.frame_shape) * dtype.itemsize
+        stream = cai.get("stream", 1) if int(cai.get("version", 2)) >= 3 else 1
+        self.stream = 0 if stream is None else int(stream)
+
+    def check(self, headers: Dict[int, Optional[tuple]]) -> None:
+        """Raises ValueError when a frame's header -- (h, w, sample bytes, channels or None when its payload does not say) -- does not
+        match out.  A frame without a readable header (None) raises its own error when the decode reaches it."""
+        h, w = self.frame_shape[:2]
+        ch = self.frame_shape[2] if len(self.frame_shape) == 3 else 1
+        for i, hdr in headers.items():
+            if hdr is not None and (hdr[:3] != (h, w, self.dtype.itemsize) or hdr[3] not in (None, ch)):
+                raise ValueError(f"frame {i} is {hdr[0]} x {hdr[1]} x {hdr[3] or '?'} of {hdr[2]}-byte samples; out holds "
+                                 f"{self.frame_shape} of {self.dtype}")
+
+    def frame(self, data: np.ndarray, i: int) -> np.ndarray:
+        if data.shape != self.frame_shape or data.dtype != self.dtype:
+            raise ValueError(f"frame {i} is {data.shape} {data.dtype}; out holds {self.frame_shape} {self.dtype}")
+        return data
+
+    def put(self, st: FrameStream, slot: int, count: int, index: int) -> None:
+        """Stream slots slot .. slot+count-1 to file frames index .. index+count-1 of out."""
+        st.copy_frames(slot, count, self.ptr + (index - self.start) * self.frame_bytes, (self.stop - index) * self.frame_bytes,
+                       self.stream)
+
+
 class ImprovedVideoCompressor:
     """ivc.ImprovedVideoCompressor (ivc:309-523) with the GOP loop wired in.
 
@@ -714,10 +793,12 @@ class ImprovedVideoCompressor:
             raise _cabi.RbfError(f"corrupt inter frame: k = {p.k}")
 
     @staticmethod
-    def _decode_group(st: FrameStream, base: int, group: List["_InterJob"]) -> np.ndarray:
+    def _decode_group(st: FrameStream, base: int, group: List["_InterJob"], skip: int = 0, out: "_DeviceOut" = None,
+                      index: int = 0) -> Optional[np.ndarray]:
         """Frames base+1 .. base+len(group) of `st` (slots modulo st.max_frames) from frame `base` and the group's payloads: one
-        decode_masks, one apply_chain (value modes and motion fields included) and one download_batch.  Raises the first bad frame's
-        error."""
+        decode_masks, one apply_chain (value modes and motion fields included) and one download_batch of all but the first `skip`
+        frames, which stay on the device (None when that is all of them).  With `out`, those frames go to its device buffer as file
+        frames index+skip .. instead, through one copy_frames, and None is returned.  Raises the first bad frame's error."""
         m, n = len(group), st.npix
         raws = [bool(j.p.raw) for j in group]
         nbs = [(n + 7) // 8 if r else (j.l + 7) // 8 for j, r in zip(group, raws)]
@@ -744,7 +825,12 @@ class ImprovedVideoCompressor:
         applied = st.apply_chain(base, **vals, modes=[j.p.vmode for j in group], motion=[j.field_arr for j in group])
         if not np.array_equal(applied, ones):
             raise ValueError(f"corrupt inter frame: {applied.tolist()} pixels applied, {ones.tolist()} expected")
-        return st.download_batch((base + 1) % st.max_frames, m)
+        if skip >= m:
+            return None
+        if out is not None:
+            out.put(st, (base + 1 + skip) % st.max_frames, m - skip, index + skip)
+            return None
+        return st.download_batch((base + 1 + skip) % st.max_frames, m - skip)
 
     @staticmethod
     def _inflate_group(st: FrameStream, jobs: List["_InterJob"], pool) -> None:
@@ -763,34 +849,62 @@ class ImprovedVideoCompressor:
         for j in dev:
             j.values = pool.submit(zlib.decompress, j.p.vz)
 
-    def _decode_run(self, run: List["_InterJob"], prev, streams: Dict[tuple, FrameStream], pool) -> list:
-        """The frames of a run of consecutive inter payloads that follows `prev`, in groups of batch_size.  The run's base frame is
-        uploaded once; each group chains from the previous group's last frame, which stays on the device."""
-        pdata = np.ascontiguousarray(_frame_data(prev))
+    def _decode_span(self, inter: List[bool], jobs: "_Jobs", k: int, start: int, stop: int, streams: Dict[tuple, FrameStream],
+                     pool, out: "_DeviceOut" = None):
+        """Decodes payloads [k, stop) and yields the frames [start, stop) (k <= start: the last keyframe at or before start, or 0),
+        one list per keyframe and per group; with `out`, writes them to its device buffer instead and yields their count.
+        inter[i]: payload i is an inter payload.  Each run of inter payloads is rebuilt from the keyframe before it in groups of
+        batch_size counted from the run's first frame, as in a whole-file decode.  The run's base frame is uploaded once; each group
+        chains from the previous group's last frame, which stays on the device, and frames before start are never downloaded.  The
+        first bad frame of [k, stop) raises, after the frames before it have been yielded."""
         group_size = max(1, int(self.batch_size))
-        out, st, base = [], None, 0
-        for g0 in range(0, len(run), group_size):
-            group, err = [], None
-            if any(j.p is not None and j.values is None for j in run[g0:g0 + group_size]):
-                if st is None:
-                    st = self._run_stream(pdata, group_size, streams)
-                self._inflate_group(st, run[g0:g0 + group_size], pool)
-            for job in run[g0:g0 + group_size]:
-                try:
-                    self._check_inter(job, pdata)
-                except Exception as e:                       # the frames before it are decoded first: their errors come first
-                    err = e
-                    break
-                group.append(job)
-            if group:
-                if st is None:
-                    st = self._run_stream(pdata, group_size, streams)
-                dec = self._decode_group(st, base, group)
-                base = (base + len(group)) % st.max_frames
-                out += [YUVFrame(f) if hasattr(prev, "yuv_info") else f for f in dec]
-            if err is not None:
-                raise err
-        return out
+        prev = st = pdata = None
+        base, i = 0, k
+        while i < stop:
+            if not inter[i]:                                 # a keyframe: built on the host; a run after it starts from it
+                prev, st, base = jobs.take(i).result(), None, 0
+                pdata = np.ascontiguousarray(_frame_data(prev))
+                if i >= start:
+                    if out is None:
+                        yield [prev]
+                    else:                                    # through the slot the run after it would upload it to
+                        st = self._run_stream(out.frame(pdata, i), group_size, streams)
+                        out.put(st, 0, 1, i)
+                        yield 1
+                i += 1
+                continue
+            if prev is None:
+                raise ValueError("inter frame without a preceding frame")
+            end = i
+            while end < stop and inter[end]:
+                end += 1
+            for g0 in range(i, end, group_size):
+                run = [jobs.take(j) for j in range(g0, min(g0 + group_size, end))]
+                group, err = [], None
+                if any(j.p is not None and j.values is None for j in run):
+                    if st is None:
+                        st = self._run_stream(pdata, group_size, streams)
+                    self._inflate_group(st, run, pool)
+                for job in run:
+                    try:
+                        self._check_inter(job, pdata)
+                    except Exception as e:                   # the frames before it are decoded first: their errors come first
+                        err = e
+                        break
+                    group.append(job)
+                if group:
+                    if st is None:
+                        st = self._run_stream(pdata, group_size, streams)
+                    skip = max(0, start - g0)
+                    dec = self._decode_group(st, base, group, skip, out, g0)
+                    base = (base + len(group)) % st.max_frames
+                    if skip < len(group):
+                        yield len(group) - skip if out is not None else \
+                            [YUVFrame(f) if hasattr(prev, "yuv_info") else f for f in dec]
+                    dec = None                               # a reader holds one group of decoded frames, not two
+                if err is not None:
+                    raise err
+            i = end
 
     @staticmethod
     def _run_stream(pdata: np.ndarray, group_size: int, streams: Dict[tuple, FrameStream]) -> FrameStream:
@@ -828,8 +942,8 @@ class ImprovedVideoCompressor:
 
     def decompress_video(self, input_path: str = None, output_path: Optional[str] = None,
                          compressed_frames: List[bytes] = None, metadata: Dict = None) -> List[np.ndarray]:
-        """ivc:452-504.  Each run of inter frames is rebuilt on the GPU in groups of batch_size (_decode_run).  zlib streams of the
-        GPU entropy coder (78 9C: keyframe blobs, changed values) are inflated on the GPU -- a group's value streams straight into
+        """ivc:452-504.  Each run of inter frames is rebuilt on the GPU in groups of batch_size (_decode_span over the whole file;
+        VideoReader runs the same driver over a span).  zlib streams of the GPU entropy coder (78 9C: keyframe blobs, changed values) are inflated on the GPU -- a group's value streams straight into
         the buffer its reconstruction reads; every other zlib stream (CPU zlib's 78 DA, raw masks, motion fields), and any stream
         the GPU declines, is inflated with zlib.decompress in a pool of num_threads."""
         if input_path and os.path.exists(input_path):                              # ivc:471-485
@@ -849,21 +963,12 @@ class ImprovedVideoCompressor:
         streams: Dict[tuple, FrameStream] = {}
         pool = ThreadPoolExecutor(self.num_threads)
         try:
-            jobs = [self._start_inter(c, pool) if c[:len(_INTER_TAG)] in _INTER_TAGS else self._start_key(c, pool)
-                    for c in compressed_frames]
-            i = 0
-            while i < len(jobs):
-                if not isinstance(jobs[i], _InterJob):
-                    frames.append(jobs[i].result())
-                    i += 1
-                    continue
-                if not frames:
-                    raise ValueError("inter frame without a preceding frame")
-                j = i
-                while j < len(jobs) and isinstance(jobs[j], _InterJob):
-                    j += 1
-                frames += self._decode_run(jobs[i:j], frames[-1], streams, pool)
-                i = j
+            count = len(compressed_frames)
+            inter = [_is_inter(c) for c in compressed_frames]
+            jobs = _Jobs(self, compressed_frames.__getitem__, inter, pool, count)
+            jobs.start(count)                                # every payload's inflates start up front
+            for part in self._decode_span(inter, jobs, 0, 0, count, streams, pool):
+                frames += part
         finally:
             pool.shutdown(wait=True, cancel_futures=True)
             for st in streams.values():
@@ -896,3 +1001,164 @@ class ImprovedVideoCompressor:
             out.write(d)
         out.release()
         return output_path
+
+
+def _frame_header(payload, inter: bool) -> Optional[tuple]:
+    """(h, w, sample bytes, channels) of a payload without decoding it; channels is None for a keyframe, whose layout does not
+    carry it.  None when the layout cannot be read: the decode raises that payload's error."""
+    try:
+        if inter:
+            p = ImprovedVideoCompressor._parse_inter(payload)
+            return p.h, p.w, p.isz, p.ch
+        return struct.unpack_from("<III", payload, 0) + (None,)
+    except Exception:
+        return None
+
+
+class VideoReader:
+    """Random access to a compressed video: any frame range decoded from the last keyframe at or before it.
+
+        r = VideoReader(source, compressor=None)   # a BFVC path, or a sequence of payloads (decompress_video's compressed_frames)
+        len(r); r.keyframes                        # frame count; indices of the keyframe payloads
+        r.read(start, stop, out=None)              # == decompress_video(...)[start:stop]; with out=, into device memory
+        r[i]; r[a:b]; for f in r: ...; with VideoReader(path) as r: ...
+
+    `compressor` (default ImprovedVideoCompressor()) decodes, with its batch_size and num_threads.  Opening a file reads its
+    length table and the first 8 bytes of every payload, which say whether it is a keyframe; a read of [start, stop) reads, parses
+    and inflates payloads [k, stop) only, k the last keyframe at or before start, and raises what decompress_video raises for the
+    first bad frame among them.  Frames before start are rebuilt on the device and never downloaded.  Iteration decodes one group
+    at a time, reading the next group's payloads ahead.  close() releases the file and the device streams."""
+
+    def __init__(self, source, compressor: Optional[ImprovedVideoCompressor] = None):
+        self._comp = compressor if compressor is not None else ImprovedVideoCompressor()
+        self._fh = self._src = None
+        self._streams: Dict[tuple, FrameStream] = {}         # of read(): kept for the next read, released by close()
+        self._live: List[Dict[tuple, FrameStream]] = []     # of iterators not yet finished
+        if isinstance(source, (str, os.PathLike)):
+            self._open(os.fspath(source))
+        else:
+            self._src = source
+            self._inter = [_is_inter(source[i]) for i in range(len(source))]
+        if not self._inter:
+            self.close()
+            raise ValueError("No compressed frames provided")
+        self.keyframes = [i for i, x in enumerate(self._inter) if not x]
+
+    def _open(self, path: str) -> None:
+        """Reads the magic, the count and the length table, seeking from length prefix to length prefix, and each payload's
+        first 8 bytes.  A payload cut short by the end of the file is read as short as it is there."""
+        self._fh = open(path, "rb")
+        magic = self._fh.read(4)
+        if magic != b"BFVC":
+            self.close()
+            raise ValueError(f"Invalid file format: {magic}")
+        try:
+            count = struct.unpack("<I", self._fh.read(4))[0]
+            self._spans, self._inter, pos = [], [], 8
+            for _ in range(count):
+                self._fh.seek(pos)
+                size = struct.unpack("<I", self._fh.read(4))[0]
+                self._inter.append(_is_inter(self._fh.read(min(size, len(_INTER_TAG)))))
+                self._spans.append((pos + 4, size))
+                pos += 4 + size
+        except BaseException:
+            self.close()
+            raise
+
+    def _payload(self, i: int):
+        if self._src is not None:
+            return self._src[i]
+        if self._fh is None:
+            raise ValueError("the reader is closed")
+        off, size = self._spans[i]
+        self._fh.seek(off)
+        return self._fh.read(size)
+
+    def __len__(self) -> int:
+        return len(self._inter)
+
+    def _decode(self, k: int, start: int, stop: int, payload, streams: Dict[tuple, FrameStream], out: "_DeviceOut" = None,
+                ahead: Optional[int] = None):
+        """_decode_span over payloads [k, stop): all started at once (ahead None), or each group's while the one before is decoded."""
+        from concurrent.futures import ThreadPoolExecutor
+        pool = ThreadPoolExecutor(self._comp.num_threads)
+        try:
+            jobs = _Jobs(self._comp, payload, self._inter, pool, stop, ahead or 0)
+            if ahead is None:
+                jobs.start(stop, k)
+            yield from self._comp._decode_span(self._inter, jobs, k, start, stop, streams, pool, out)
+        finally:
+            pool.shutdown(wait=True, cancel_futures=True)
+
+    def read(self, start: int, stop: int, out=None):
+        """decompress_video(...)[start:stop], decoded from the last keyframe at or before start.  With `out` -- an object with
+        __cuda_array_interface__ of shape (stop - start, H, W) or (stop - start, H, W, C), the frames' dtype, C-contiguous, on the
+        library's device -- the frames' samples are written there instead and `out` is returned: keyframes through an upload into a
+        device slot, inter frames straight from the slots they are rebuilt in, one copy per group; YUV planes are not produced.  A
+        mismatched `out` raises ValueError before anything is launched."""
+        start, stop, n = operator.index(start), operator.index(stop), len(self)
+        if not 0 <= start <= stop <= n:
+            raise IndexError(f"frames [{start}, {stop}) outside [0, {n}]")
+        dev = None if out is None else _DeviceOut(out, start, stop)
+        if start == stop:
+            return [] if out is None else out
+        at = bisect.bisect_right(self.keyframes, start)
+        k = self.keyframes[at - 1] if at else 0
+        payloads = {i: self._payload(i) for i in range(k, stop)}
+        if dev is not None:
+            dev.check({i: _frame_header(payloads[i], self._inter[i]) for i in range(start, stop)})
+        frames: list = []
+        for part in self._decode(k, start, stop, payloads.__getitem__, self._streams, dev):
+            if dev is None:
+                frames += part
+        return frames if dev is None else out
+
+    def __getitem__(self, key):
+        if isinstance(key, slice):
+            a, b, step = key.indices(len(self))
+            if step != 1:
+                raise ValueError(f"slice step must be 1, not {step}")
+            return self.read(a, max(a, b))
+        i = operator.index(key)
+        if i < 0:
+            i += len(self)
+        if not 0 <= i < len(self):
+            raise IndexError(f"frame index {key} out of range for {len(self)} frames")
+        return self.read(i, i + 1)[0]
+
+    def __iter__(self):
+        """Every frame in order, as decompress_video returns them; holds one group of decoded frames at a time."""
+        streams: Dict[tuple, FrameStream] = {}
+        self._live.append(streams)
+        parts = self._decode(0, 0, len(self), self._payload, streams, ahead=max(1, int(self._comp.batch_size)))
+        try:
+            for part in parts:
+                part.reverse()
+                while part:
+                    yield part.pop()
+        finally:
+            parts.close()
+            for st in streams.values():
+                st.close()
+            self._live = [s for s in self._live if s is not streams]
+
+    def close(self) -> None:
+        for streams in [self._streams] + self._live:
+            for st in streams.values():
+                st.close()
+            streams.clear()
+        if self._fh is not None:
+            self._fh.close()
+            self._fh = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

@@ -294,6 +294,13 @@ class FrameStream:
         _cabi.check(_cabi.lib().rbf_stream_download_batch(self._h, int(first), int(count), _cabi.ptr(out)), _cabi.ctx())
         return out
 
+    def copy_frames(self, first: int, count: int, ptr: int, capacity: int, stream: int = 0) -> None:
+        """download_batch into device memory: frames first .. first+count-1 (slots modulo max_frames) to the device address `ptr`,
+        back to back, `capacity` bytes at most.  `stream` (a __cuda_array_interface__ v3 stream: 0 none, 1 legacy default, 2
+        per-thread default, else a cudaStream_t) is waited for before the buffer is written; returns when the copy is done."""
+        _cabi.check(_cabi.lib().rbf_stream_copy_frames(self._h, int(first), int(count), C.c_void_p(int(ptr) or None), int(capacity),
+                                                       int(stream)), _cabi.ctx())
+
     def stage_ms(self) -> dict:
         out = (C.c_double * 6)()
         _cabi.check(_cabi.lib().rbf_stream_stage_ms(self._h, out), _cabi.ctx())
